@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- SAM-PT hot path throughput on B200 (contract: see the task brief / DESIGN.md §measurement).
+"""bench.py -- SAM-PT hot path throughput on one H100 (DESIGN.md §measurement).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2|C1|...]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2|C1|...] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path (PIPS track -> SAM ViT encode -> prompt+mask decode with 12 refinements) over one
 synthetic clip.  Headline workload = BASELINE config C2: 50 frames 480x854, SAM ViT-H + PIPS, 1 mask x 8 positive points.
@@ -10,6 +10,10 @@ synthetic clip.  Headline workload = BASELINE config C2: 50 frames 480x854, SAM 
            region) and the result summary (scores + trajectories + visibilities) read back D2H.
 `--impl reference`: the reference's own CPU path (oracle port: reference PIPS restated + SAM restated, torch CPU, all host
            threads) on a bounded sample of the same workload.
+`--dump-outputs DIR`: after the timed steps, the arrays the last resident step returned (trajectories, visibilities, per-frame
+           scores, and a fixed seeded sample of the mask logits) are written as DIR/<name>.npy so that two builds can be
+           compared output for output; inputs and weights are seeded, so they are identical from run to run.  The -inf of
+           an empty mask is written as a finite stand-in and flagged in DIR/<name>_empty.npy (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -50,12 +54,18 @@ COT_VIS_BIAS = 0.6   # synth.condition_cotracker: ~90 % of the C3 / C5 query poi
 
 
 def _peaks():
+    """Peaks the roofline fractions divide by: MEASURED_PEAKS.json when present, else NVIDIA's H100 SXM data sheet (dense, for
+    a card allowed 700 W; a power-limited card reaches less).  A data-sheet figure is a ceiling, never a measured rate."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"hbm_gbs": d.get("hbm_gbs", 6650.0), "bf16_tflops": d.get("bf16_tflops", 1590.0),
-                "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 1400.0), "src": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback (B200_PROFILING.md)"}
+        return {"hbm_gbs": d.get("hbm_gbs", 3350.0), "bf16_tflops": d.get("bf16_tflops", 989.0),
+                "bf16_tflops_sustained": d.get("bf16_tflops_sustained"), "src": "measured (MEASURED_PEAKS.json)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": None, "src": "H100 SXM data sheet (dense, 700 W)"}
+
+
+def _frac(a, b):
+    return a / b if b else None
 
 
 class ClockSampler:
@@ -150,7 +160,7 @@ def run_ours(args):
     frames_host = torch.stack(video["image"]).pin_memory()
     q_host = video["query_points"].pin_memory()
     ctx = native.get_context(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > L2 (126 MB): flushed between timed iterations
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > L2 (50 MB): flushed between timed iterations
 
     def step_resident(frames_dev, q_dev):
         traj, vis, logits, scores, spf = model._forward(frames_dev, q_dev)
@@ -176,11 +186,13 @@ def run_ours(args):
         for i in range(args.steps):
             flush.fill_(i & 0xFF)
             ev[i][0].record()
-            step_resident(frames_dev, q_dev)
+            last = step_resident(frames_dev, q_dev)
             ev[i][1].record()
         barrier()
     ms = sum(a.elapsed_time(b) for a, b in ev)
     launches = ctx.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     # ---------------- timed: end to end through SamPt.forward with HOST inputs + D2H result summary
     video_host = dict(video)
     video_host["image"] = [f for f in frames_host]
@@ -208,7 +220,7 @@ def run_ours(args):
     breakdown = stage_breakdown(model, frames_dev, q_dev) if args.breakdown else None
     if args.kernel_table and rank == 0:
         kernel_table(lambda: step_resident(frames_dev, q_dev), args.kernel_table)
-    # ---------------- roofline of the dominant kernel (ViT tcgen05 GEMM), measured live with CUDA events
+    # ---------------- roofline of the dominant kernel (ViT tensor-core GEMM), measured live with CUDA events
     roof = gemm_roofline(model, dev, args)
     if rank == 0 and world == 1:
         roof["in_step"] = in_step_share(lambda: step_resident(frames_dev, q_dev), T, vit)
@@ -317,6 +329,41 @@ def run_ours_frame_sharded(args, model, dev, rank, world, local):
     dist.destroy_process_group()
 
 
+DUMP_LOGITS_SAMPLE = 1 << 22   # logits elements kept by --dump-outputs (16 MB of float32; a C2 clip has 20.5 M)
+
+
+DUMP_EMPTY_FILL = -1.0e4   # finite stand-in for the -inf of an empty mask in the dumped arrays (flagged in <name>_empty.npy)
+
+
+def dump_outputs(path, result):
+    """result = (logits, scores_per_frame, trajectories, visibilities) of one step -> path/<name>.npy (float32).  The logits
+    are sampled at fixed, seeded positions (the same for every run of the same configuration).  A frame whose query points are
+    all invisible has an empty mask: its logits and score are -inf, as in the reference (sam_pt.py:766).  The dump stays
+    finite and lossless: such entries are written as DUMP_EMPTY_FILL and marked 1 in <name>_empty.npy.  Any other non-finite
+    output (NaN, +inf) is an error."""
+    import numpy as np
+    logits, spf, traj, vis = result
+    os.makedirs(path, exist_ok=True)
+    flat = logits.detach().float().reshape(-1)
+    if flat.numel() > DUMP_LOGITS_SAMPLE:
+        g = torch.Generator(device="cpu").manual_seed(0)
+        idx = torch.randperm(flat.numel(), generator=g)[:DUMP_LOGITS_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    arrays = {"logits_sample": flat, "scores_per_frame": spf, "trajectories": traj, "visibilities": vis}
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy().astype(np.float32)
+        empty = np.isneginf(a)
+        bad = ~np.isfinite(a) & ~empty
+        if bad.any():
+            raise RuntimeError(f"--dump-outputs: {name} has {int(bad.sum())} NaN / +inf values")
+        if name in ("logits_sample", "scores_per_frame"):
+            np.save(os.path.join(path, name + "_empty.npy"), empty.astype(np.float32))
+            a = np.where(empty, np.float32(DUMP_EMPTY_FILL), a)
+        elif empty.any():
+            raise RuntimeError(f"--dump-outputs: {name} has {int(empty.sum())} -inf values")
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def kernel_table(step_fn, path):
     """Per-kernel device time of one step via CUPTI (torch.profiler sees every kernel of the process, including the ones
     launched through the C ABI).  Not a bench value; written for profiles/."""
@@ -341,7 +388,7 @@ def kernel_table(step_fn, path):
             f.write(f"| `{k[:110]}` | {c} | {t / 1e3:.2f} | {t / c:.1f} | {100 * t / tot:.1f}% |\n")
 
 
-def in_step_share(step_fn, frames_per_step, vit, pattern="gemm_tc2_kernel"):
+def in_step_share(step_fn, frames_per_step, vit, pattern="gemm_tc_kernel"):
     """Cross-check of the isolated roofline timing against the real step (VERDICT r1 #4): one extra, untimed step under CUPTI
     (torch.profiler); all launches of the dominant kernel are summed.  `achieved_algorithmic` uses SURVEY §8d's 5.48 TFLOP of
     linear-layer work per ViT-H frame (what the reference computes; the padding-window skip removes ~8 % of it from the launches)."""
@@ -368,7 +415,7 @@ def in_step_share(step_fn, frames_per_step, vit, pattern="gemm_tc2_kernel"):
         if vit == "vit_h" and ker > 0:
             pk = _peaks()
             ach = frames_per_step * 5.48 / (ker / 1e6)   # TFLOP / s
-            out.update({"achieved_algorithmic": ach, "unit": "TFLOP/s", "frac_of_sustained_peak": ach / pk["bf16_tflops_sustained"],
+            out.update({"achieved_algorithmic": ach, "unit": "TFLOP/s", "frac_of_sustained_peak": _frac(ach, pk["bf16_tflops_sustained"]),
                         "frac_of_burst_peak": ach / pk["bf16_tflops"]})
         return out
     except Exception as e:   # a profiler problem must never cost the bench line
@@ -415,20 +462,7 @@ def stage_breakdown(model, frames_dev, q_dev):
     return {k: round(v, 3) for k, v in out.items()}
 
 
-def _ncu_traffic(key):
-    """DRAM bytes per launch (read + write) of a roofline kernel from the committed `ncu --set full` capture
-    (profiles/r02_roofline_traffic.json, else r01; produced by tools/ncu_targets.py + profiles/extract_traffic.py); None if absent."""
-    e = None
-    for name in ("r02_roofline_traffic.json", "r01_roofline_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            e = json.load(open(p)).get(key)
-            if e is not None:
-                break
-    return None if e is None else e["dram_read_bytes"] + e["dram_write_bytes"]
-
-
-ROOFLINE_WARM, ROOFLINE_REPS = 3, 10   # tools/ncu_targets.py lowers both so that one ncu --set full capture stays small
+ROOFLINE_WARM, ROOFLINE_REPS = 3, 10
 
 
 def corr_roofline(dev, n_points=292):
@@ -466,13 +500,10 @@ def corr_roofline(dev, n_points=292):
     nbytes = n_points * S * 4 * 64 * 128 * 4 + n_points * S * 196 * 4
     pk = _peaks()
     gbs = nbytes / (ms * 1e-3) / 1e9
-    traffic = _ncu_traffic("pips_corr")
     return {"bound": "hbm", "kernel": "pips_corr_kernel (the tracker's fused correlation gather + mixer-row assembly, N=%d points; the "
                                      "timed call adds a 1.8 MB strided copy-out of the 196 correlation columns)" % n_points,
-            "achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs / pk["hbm_gbs"], "traffic": traffic, "ms": ms,
-            # the 8x8 patches of neighbouring levels / slots overlap: most of the N x 1 MiB "minimal formulation" is served by L2.
-            # frac_dram = what actually crossed the HBM interface (ncu dram bytes of the same launch) / time / peak
-            "frac_dram": (traffic / (ms * 1e-3) / 1e9 / pk["hbm_gbs"]) if traffic else None,
+            # the 8x8 patches of neighbouring levels / slots overlap: part of the N x 1 MiB "minimal formulation" is served by L2
+            "achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs / pk["hbm_gbs"], "ms": ms,
             "peak_source": pk["src"], "algorithmic_bytes": nbytes, "l2": "flushed before every launch"}
 
 
@@ -481,7 +512,8 @@ def attn_roofline(dev, frames=10, nheads=16, hd=80):
     windowed: 25 windows x 16 heads per frame, 14x14 = 196 tokens (operands pre-extended: DK = 80 + 2*14 -> 128);
     global  : 16 heads per frame, 64x64 = 4096 tokens (DK = 80 + 2*64 -> 256).
     Algorithmic FLOPs (SURVEY §8d) = 4 * L^2 * hd per (window, head): the QK^T and P.V contractions at the true head dim, without
-    the rel-pos extension columns or tile padding; `issued` counts what the tensor pipe executes (DK-wide QK^T, 128-row tiles)."""
+    the rel-pos extension columns or tile padding; `issued` counts what the tensor pipe executes (DK-wide QK^T, 128-row query tiles,
+    64-key tiles)."""
     from ctypes import c_int
     from sampt_b200 import native
     ctx = native.get_context(dev)
@@ -516,13 +548,13 @@ def attn_roofline(dev, frames=10, nheads=16, hd=80):
         ms = e0.elapsed_time(e1) / n
         alg = 4.0 * L * L * hd * BH
         mt = ((L + 127) // 128) * 128
-        issued = 2.0 * mt * (((L + NT - 1) // NT) * NT) * (DK + hd) * BH
+        issued = 2.0 * mt * (((L + 63) // 64) * 64) * (DK + hd) * BH
         ach = alg / (ms * 1e-3) / 1e12
         out[name] = {"bound": "tensor", "kernel": "attention (ViT-H %s, %d (window, head) units of %d tokens)" % (name, BH, L), "achieved": ach,
                      "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops"],
                      "achieved_issued": issued / (ms * 1e-3) / 1e12, "frac_issued": issued / (ms * 1e-3) / 1e12 / pk["bf16_tflops"], "ms": ms,
                      "algorithmic_flops": alg, "operands_bytes": int(Q.numel() * 2 * 2 + V.numel() * 2 + o.numel() * 2),
-                     "traffic": _ncu_traffic("attn_" + name), "peak_source": pk["src"] + ", burst"}
+                     "peak_source": pk["src"]}
         del Q, K, V, o
     return out
 
@@ -581,11 +613,11 @@ def gemm_roofline(model, dev, args):
             "frac": ach / pk["bf16_tflops"],                                    # ALGORITHMIC flops (2*M*N*K) / time / measured peak
             "achieved_issued": flops_exec / (ms * 1e-3) / 1e12,                 # tensor-core work issued incl. the split-precision passes
             "frac_issued": flops_exec / (ms * 1e-3) / 1e12 / pk["bf16_tflops"],
-            # the same two against the SUSTAINED peak (cuBLAS back to back under the power cap), for reference next to the burst figure
-            "peak_sustained": pk["bf16_tflops_sustained"], "frac_of_sustained": ach / pk["bf16_tflops_sustained"],
-            "frac_issued_of_sustained": flops_exec / (ms * 1e-3) / 1e12 / pk["bf16_tflops_sustained"],
-            "traffic": _ncu_traffic("gemm_tc_kernel"), "algorithmic_bytes": 2.0 * (M * K * asp + N * K * bsp + M * N),
-            "peak_source": pk["src"] + ", burst", "shape": [M, N, K], "passes": ("1 fp16 + 2 e4m3 (= 2 fp16-pass equivalents)" if f8c else p), "ms": ms}
+            # the same two against a SUSTAINED peak (measured back to back under the power cap) when MEASURED_PEAKS.json gives one
+            "peak_sustained": pk["bf16_tflops_sustained"], "frac_of_sustained": _frac(ach, pk["bf16_tflops_sustained"]),
+            "frac_issued_of_sustained": _frac(flops_exec / (ms * 1e-3) / 1e12, pk["bf16_tflops_sustained"]),
+            "algorithmic_bytes": 2.0 * (M * K * asp + N * K * bsp + M * N),
+            "peak_source": pk["src"], "shape": [M, N, K], "passes": ("1 fp16 + 2 e4m3 (= 2 fp16-pass equivalents)" if f8c else p), "ms": ms}
 
 
 def usable_cores(cap=16):
@@ -681,6 +713,8 @@ def main():
     ap.add_argument("--kernel-table", default=None, help="write a per-kernel time table of one step (CUPTI) to this path")
     ap.add_argument("--mgpu-mode", default="frame_shard", choices=["frame_shard", "clip_per_gpu"])
     ap.add_argument("--clips-per-step", type=int, default=0, help="N > 1: clips per step (default: one per rank; C5: a single clip)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (single-GPU clip path)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* libsampt_b200.so — C ABI of the B200-native SAM-PT hot path.
+/* libsampt_b200.so — C ABI of the H100-native SAM-PT hot path.
  *
  * The reference (SysCV/sam-pt) has NO FFI: its seam is Python classes named in Hydra YAML (SURVEY.md §8b).  This
  * library sits BEHIND drop-in replacements of those classes (sam-pt_b200/sam_pt, sam-pt_b200/segment_anything[_hq])
@@ -85,11 +85,11 @@ int sampt_pips_corr_lookup(sampt_ctx* ctx, const float* fmaps, const float* l1, 
 int sampt_linear_f32(sampt_ctx* ctx, const float* X, int ldx, const float* W, int ldw, const float* bias,
                      const float* residual, int ldr, float* Y, int ldy, int M, int N, int K, int act, void* stream);
 
-/* ---- tensor-core GEMM (tcgen05 / TMEM / TMA), the building block of ImageEncoderViT's Linear layers ------------- */
+/* ---- tensor-core GEMM (tensor-core / registers / TMA), the building block of ImageEncoderViT's Linear layers ------------- */
 /* C = act(A[M,K] B[N,K]^T + bias) with fp16 (bf16 if is_bf16) operands and fp32 accumulation.  Exactly one of
  * out16 (fp16/bf16 [M,ldc]) / out32 (fp32 [M,ldc], optional fp32 residual added) is non-null.
  * precision 1: single pass.  2: the weights B are carried as fp16 hi|lo halves, B = [N,2K] with lo at column K (A plain):
- * A.B_hi + A.B_lo.  3: A too (A = [M,2K]); products hi.hi + lo.hi + hi.lo accumulate in the same TMEM tile (~fp32).
+ * A.B_hi + A.B_lo.  3: A too (A = [M,2K]); products hi.hi + lo.hi + hi.lo accumulate in the same registers tile (~fp32).
  * split_off > 0 (out16 only): additionally writes lo = fp16(v - fp16(v)) at column offset split_off.
  * Replaces torch.nn.Linear inside segment_anything.modeling.image_encoder (un-vendored; call site
  * sam_pt/modeling/sam_pt.py:849 -> SamPredictor.set_image -> ImageEncoderViT.forward). */
@@ -97,20 +97,21 @@ int sampt_gemm_f16(sampt_ctx* ctx, const void* A, int lda, const void* B, int ld
                    int is_bf16, const float* bias, int act, void* out16, float* out32, const float* resid, int ldc,
                    int split_off, void* stream);
 
-/* The same product with the two CORRECTION passes in e4m3 (tcgen05.mma.kind::f8f6f4, twice the fp16 rate): the terms
+/* The same product with the two CORRECTION passes in e4m3 (e4m3 wgmma, twice the fp16 rate): the terms
  * A_lo.B_hi and A_hi.B_lo are 2^-12 of the result, so e4m3's 2^-5 rounding leaves a 2^-17 residual -- fp32-like products
  * for 2 fp16-pass equivalents instead of 3.  Rows of 2K fp16 units:
  *   A: [fp16(x) : K halves | e4m3((x - fp16(x)) * 2^12) : K bytes | e4m3(x * 2^-3) : K bytes]        (sampt_split_f8c)
  *   B: [fp16(w * 2^s) : K halves | e4m3(w * 2^(s-12)) : K bytes | e4m3((w * 2^s - fp16(w * 2^s)) * 2^3) : K bytes]
  * with s the largest exponent keeping |w| * 2^s <= 2^15; acc_scale_dev points to 2^-s.  out_f8 != 0 with split_off = N: the
- * output is written in the A layout of the next such GEMM.  Needs M >= 256, N % 256 == 0, K % 128 == 0 (CTA-pair kernel).
+ * output is written in the A layout of the next such GEMM.  Needs M >= 256, N % 256 == 0, K % 128 == 0 (the shapes of the ViT's linear layers).
  * Same role as sampt_gemm_f16 (torch.nn.Linear of the un-vendored image_encoder; call site sam_pt/modeling/sam_pt.py:849). */
 int sampt_gemm_f8c(sampt_ctx* ctx, const void* A, const void* B, int M, int N, int K, const float* acc_scale_dev, const float* bias,
                    int act, void* out16, float* out32, const float* resid, int ldc, int split_off, int out_f8, void* stream);
 int sampt_split_f8c(sampt_ctx* ctx, const float* x, int M, int K, void* out, void* stream);
 
-/* softmax(Qx Kx^T) V on tcgen05 with pre-extended operands (rel-pos folded into the contraction, see csrc/attn_tc.cu):
+/* softmax(Qx Kx^T) V on tensor cores with pre-extended operands (rel-pos folded into the contraction, see csrc/attn_tc.cu):
  * Qx [BH,Lq,DK], Kx [BH,Lk,DK], Vt [BH,HD,Lkp] fp16; out fp16 [(BH/nheads)*Lq, ld_out] with head h at columns h*HD.
+ * NT (a key-tile size) is accepted and ignored: the kernel walks the keys in tiles of 64.
  * Replaces Attention.forward + add_decomposed_rel_pos of upstream image_encoder.py. */
 int sampt_attention_f16(sampt_ctx* ctx, const void* Qx, const void* Kx, const void* Vt, int BH, int Lq, int Lk, int Lkp, int DK,
                         int HD, int NT, int nheads, void* out, int ld_out, int split_off, void* stream);

@@ -8,7 +8,7 @@
 // Round 1 computed the 2S dot products per query on the CUDA cores (440 k FMA per 14x14 window-head, fed from shared memory at
 // ~1 load per 5 FMA): 0.66 ms per 10-frame launch for 0.9 GB of traffic, 1.3 TB/s.  Here they are ONE small tensor-core product
 // per CTA:  T = q [TC x HD] . Rcat^T [HD x 2(2S-1)],  Rcat = [Rh ; Rw], as legacy mma.sync m16n8k16 tiles (the operands are tiny
-// and live in shared memory; tcgen05 + TMEM would be set-up cost only), with Rcat carried as fp16 hi + lo so that the table is
+// and live in shared memory; a wgmma pipeline would be set-up cost only), with Rcat carried as fp16 hi + lo so that the table is
 // exact to ~2^-22 -- the fp32 table of the reference -- and q as the fp16 it already is.  The shifted pick
 // Q'ext[t][j] = T[t][qy - j + S-1] is then a shared-memory gather while the rows are assembled.  Everything else is coalesced
 // 16-byte traffic, so the kernel is bound by its algorithmic bytes (read qkv once, write Q', K', V^T once).

@@ -24,7 +24,8 @@ extern "C" int sampt_ctx_create(int device, sampt_ctx** out) {
   SAMPT_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   SAMPT_CUDA(cudaGetDeviceProperties(&prop, device));
-  SAMPT_CHECK(prop.major == 10, "libsampt_b200 is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+  SAMPT_CHECK(prop.major == 9 && prop.minor == 0, "libsampt_b200 is built for sm_90a only; device %d is sm_%d%d", device, prop.major,
+              prop.minor);
   Ctx* c = new Ctx();
   c->device = device;
   c->num_sms = prop.multiProcessorCount;

@@ -1,5 +1,5 @@
 // Shared infrastructure of libsampt_b200.so: error reporting, the per-device context (weight registry +
-// bump-allocated workspace), small device helpers.  sm_100a only.
+// bump-allocated workspace), small device helpers.  sm_90a only.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -58,7 +58,7 @@ struct TensorRef {
 
 struct Ctx {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   std::unordered_map<std::string, TensorRef> tensors;  // caller-owned device memory, registered by name
   // workspace: caller-owned slab, bump allocated per pipeline call
   char* ws_base = nullptr;

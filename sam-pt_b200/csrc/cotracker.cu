@@ -1,4 +1,4 @@
-// CoTracker v1 (cotracker_stride_4_wind_8) window update on the B200, strict fp32.
+// CoTracker v1 (cotracker_stride_4_wind_8) window update on the H100, strict fp32.
 // Upstream: co-tracker @ 4f297a9, cotracker/models/core/cotracker/{cotracker.py,blocks.py}, models/core/embeddings.py
 // (un-vendored, requirements.txt:31; SURVEY Appendix B.3, PARITY UNPINNED).  Reference call sites:
 // sam_pt/point_tracker/cotracker/tracker.py:104,159 (model(rgbs, queries, iters=6)).
@@ -342,8 +342,8 @@ struct CotBufs {
   __half *h16, *att16, *mlp16;   // hi | lo operands of the tensor-core path (null: fp32 CUDA-core GEMMs)
 };
 
-// Y[M, N] (fp32, + bias, + residual) or the next operand (fp16 hi | lo, GELU-tanh) = X16 . W16^T in three tcgen05 passes
-// (A_hi.B_hi + A_lo.B_hi + A_hi.B_lo into one fp32 TMEM accumulator: products exact to ~2^-22, i.e. fp32-level like the CUDA-core
+// Y[M, N] (fp32, + bias, + residual) or the next operand (fp16 hi | lo, GELU-tanh) = X16 . W16^T in three tensor-core passes
+// (A_hi.B_hi + A_lo.B_hi + A_hi.B_lo into one fp32 register accumulator: products exact to ~2^-22, i.e. fp32-level like the CUDA-core
 // path it replaces).  The UpdateFormer is 21.5 M parameters x (8 N) token rows x 6 iterations x ~24 windows x 2 directions: at
 // N = 256 points (C5) that is 25 TFLOP per clip -- 1.2 s on the fp32 pipes, the longest serial stage of a frame-sharded C5 clip.
 static int cot_tcg(Ctx* c, cudaStream_t st, const __half* X16, const __half* W16, const float* bias, const float* resid, float* Y32,
@@ -444,7 +444,7 @@ extern "C" int sampt_cotracker_window(sampt_ctx* ctx, const float* fmaps, const 
   SAMPT_TRY(ws_get(c, &b.att, (size_t)M * CT_HID, "cot att"));
   SAMPT_TRY(ws_get(c, &b.mlp, (size_t)M * 4 * CT_HID, "cot mlp"));
   SAMPT_TRY(ws_get(c, &delta, (size_t)M * 130, "cot delta"));
-  // UpdateFormer GEMMs on tcgen05 (three fp16 hi | lo passes) once the token count fills 128-row tiles; SAMPT_COT_TC=0 keeps fp32
+  // UpdateFormer GEMMs on tensor cores (three fp16 hi | lo passes) once the token count fills 128-row tiles; SAMPT_COT_TC=0 keeps fp32
   static const int cot_tc_on = [] { const char* e = std::getenv("SAMPT_COT_TC"); return (e != nullptr && e[0] == '0') ? 0 : 1; }();
   b.h16 = b.att16 = b.mlp16 = nullptr;
   if (cot_tc_on && M >= 128 && tb[0].qkv_w16 != nullptr) {

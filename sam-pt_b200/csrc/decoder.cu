@@ -716,7 +716,7 @@ __global__ void init_ctl_kernel(int* bbox, int* skip, int* n_done) {
 // ====================================================================================================================
 struct AttnW {
   const float *qw, *qb, *kw, *kb, *vw, *vb, *ow, *ob; int internal;
-  // image-side projections on tcgen05: weights as fp16 hi|lo [N, 2K] (null: that projection is token-side only)
+  // image-side projections on tensor cores: weights as fp16 hi|lo [N, 2K] (null: that projection is token-side only)
   const __half *qw16 = nullptr, *kw16 = nullptr, *vw16 = nullptr, *ow16 = nullptr;
 };
 struct LayerW {
@@ -729,8 +729,8 @@ struct DecW {
   LayerW layer[2];
   AttnW final_attn; const float *nfw, *nfb, *pek_final;
   const float *up0_w /*[256 tok-in][4*64]^T as [4*64][256]*/, *up0_b4 /*[256] bias tiled over the 4 sub-pixels*/;
-  const __half* up0_w16 = nullptr;  // the same matrix as fp16 hi|lo [256, 512] for the tcgen05 path
-  bool tc = false;                  // image-side GEMMs (4096-row operands) on the tcgen05 split-precision GEMM
+  const __half* up0_w16 = nullptr;  // the same matrix as fp16 hi|lo [256, 512] for the tensor-core path
+  bool tc = false;                  // image-side GEMMs (4096-row operands) on the tensor-core split-precision GEMM
   const float *up_lnw, *up_lnb, *up3_w, *up3_b;
   Mlp3Job hyper[4], iou;
   DenseW dense;
@@ -839,7 +839,7 @@ static int load_dec(Ctx* c, DecW* w) {
 struct DecBufs {
   float *tokens, *queries, *qpe, *tq, *tk, *tv, *ta, *tmp, *mlp_h;   // token side  (T rows)
   float *src, *keys, *ik, *iv, *iq, *ia;                            // image side  (4096 rows)
-  __half *keys16 = nullptr, *ia16 = nullptr;                         // fp16 hi|lo copies of keys [GG,512] / ia [GG,256] (tcgen05 path)
+  __half *keys16 = nullptr, *ia16 = nullptr;                         // fp16 hi|lo copies of keys [GG,512] / ia [GG,256] (tensor-core path)
   float *u1, *hyper, *iou4, *part;
   float *u_sam, *mf1, *mf2;  // HQ only
   int T;
@@ -852,7 +852,7 @@ static int sg(Ctx* c, cudaStream_t st, const float* X, int ldx, const float* W, 
   return sgemm_nt_skip(c, st, X, ldx, W, K, b, resid, ldr, Y, ldy, M, N, K, act, skip);
 }
 
-// x [rows, K] fp32 -> out [rows, 2K] fp16: hi = fp16(x) | lo = fp16(x - hi)   (A operand of the split-precision tcgen05 GEMM)
+// x [rows, K] fp32 -> out [rows, 2K] fp16: hi = fp16(x) | lo = fp16(x - hi)   (A operand of the split-precision tensor-core GEMM)
 __global__ void __launch_bounds__(256)
 split_f32_kernel(const float* __restrict__ x, __half* __restrict__ out, long long n4 /* rows*K/4 */, int K, const int* skip) {
   SKIP_RETURN(skip);
@@ -876,8 +876,8 @@ static int split_rows(Ctx* c, cudaStream_t st, const float* x, __half* out, int 
   SAMPT_LAUNCH_CHECK();
   return 0;
 }
-// Y = X W^T + b (+ resid), X given as fp16 hi|lo [M, 2K], W as fp16 hi|lo [N, 2K]: three tcgen05 passes A_hi.B_hi + A_lo.B_hi +
-// A_hi.B_lo into one fp32 TMEM accumulator (products exact to ~2^-22: the decoder stays at fp32-level accuracy).  The residual is
+// Y = X W^T + b (+ resid), X given as fp16 hi|lo [M, 2K], W as fp16 hi|lo [N, 2K]: three tensor-core passes A_hi.B_hi + A_lo.B_hi +
+// A_hi.B_lo into one fp32 register accumulator (products exact to ~2^-22: the decoder stays at fp32-level accuracy).  The residual is
 // indexed like Y (same leading dimension).
 static int tcg(Ctx* c, cudaStream_t st, const __half* X16, const __half* W16, const float* b, const float* resid, float* Y, int ldy,
                int M, int N, int K, const int* skip) {
@@ -896,7 +896,7 @@ static int attn_tok_to_img(Ctx* c, cudaStream_t st, const AttnW& a, const float*
                            DecBufs& b, float* out /*[T,256]*/, const float* resid, int GG, const int* skip) {
   const int T = b.T;
   SAMPT_TRY(sg(c, st, q_in, 256, a.qw, a.qb, nullptr, 0, b.tq, 128, T, 128, 256, 0, skip));
-  if (a.kw16 != nullptr) {   // tcgen05: b.keys16 holds the hi|lo split of `keys` (kept in sync by the caller)
+  if (a.kw16 != nullptr) {   // tensor cores: b.keys16 holds the hi|lo split of `keys` (kept in sync by the caller)
     SAMPT_TRY(tcg(c, st, b.keys16, a.kw16, a.kb, pek, b.ik, 128, GG, 128, 256, skip));           // (keys + key_pe) Wk^T
     SAMPT_TRY(tcg(c, st, b.keys16, a.vw16, a.vb, nullptr, b.iv, 128, GG, 128, 256, skip));
   } else {

@@ -1,15 +1,17 @@
 // Tensor-core GEMM for the SAM ViT encoder:  C[M,N] = epilogue( A[M,K] . B[N,K]^T ),  fp16/bf16 operands, fp32 accumulate.
 //
-// sm_100a design (one CTA per SM, persistent over 128x256 output tiles):
-//   warp 0      TMA producer   : cp.async.bulk.tensor 2-D boxes (64 halves x rows, 128B swizzle) into a 4-stage smem ring
-//   warp 1      MMA issuer     : one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=256, K=16), fp32
-//                                accumulators in TMEM (2 x 256 columns, double buffered so the epilogue of tile i overlaps
-//                                the main loop of tile i+1); tcgen05.commit releases smem stages / publishes accumulators
-//   warps 2..5  epilogue       : tcgen05.ld (32 lanes x 32 columns) -> bias / GELU / residual / fp16|fp32|split store
+// sm_90a design (one CTA per 128x128 output tile, 288 threads):
+//   warp 8          TMA producer : cp.async.bulk.tensor 2-D boxes (64 halves x rows, 128B swizzle) into a 5-stage smem ring,
+//                                  completion on per-stage mbarriers
+//   warpgroups 0,1  consumers    : wgmma.mma_async m64n128 (k16 fp16/bf16, k32 e4m3) on 64 rows each, fp32 accumulators in
+//                                  registers, one k-block in flight; then bias / GELU / residual / fp16|fp32|split store
 //
 // "Split" precision (accuracy dial, DESIGN.md §precision): an operand x is carried as fp16 hi + fp16 lo
 // (lo = fp16(x - hi)); the K loop then runs over up to three segments  A_hi.B_hi + A_lo.B_hi + A_hi.B_lo  accumulating
-// into the same TMEM tile.  Segments are described by column offsets into the A / B matrices, so the kernel is the same.
+// into the same registers.  Segments are described by column offsets into the A / B matrices, so the kernel is the same.
+// e4m3 segments (precision 6, tc_api.cuh) accumulate into a SEPARATE register tile that is added in the epilogue: wgmma's
+// fp8 accumulation does not keep full fp32 precision, which is harmless for the 2^-12-sized correction terms alone but would
+// round away the low bits of the fp16 main product if they shared one accumulator.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "kernels.cuh"
@@ -20,191 +22,150 @@ namespace sampt {
 
 using namespace tc;
 
-constexpr int G_BM = 128, G_BN = 256, G_BK = 64, G_STAGES = 4;
+constexpr int G_BM = 128, G_BN = 128, G_BK = 64, G_STAGES = 5;
 constexpr int G_A_BYTES = G_BM * G_BK * 2;  // 16 KB
-constexpr int G_B_BYTES = G_BN * G_BK * 2;  // 32 KB
+constexpr int G_B_BYTES = G_BN * G_BK * 2;  // 16 KB
 constexpr int G_STAGE_BYTES = G_A_BYTES + G_B_BYTES;
 constexpr int G_SMEM_BYTES = G_STAGES * G_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-constexpr int G_THREADS = 192;
+constexpr int G_THREADS = 288;
 
+template <bool F8>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
                GemmSeg seg, GemmEpi ep) {
-  if (ep.skip != nullptr && *ep.skip != 0) return;   // uniform over the grid: nothing has been allocated yet
+  if (ep.skip != nullptr && *ep.skip != 0) return;   // uniform over the grid
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + G_STAGES * G_STAGE_BYTES);
   uint64_t* empty_bar = full_bar + G_STAGES;
-  uint64_t* tfull_bar = empty_bar + G_STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (M + G_BM - 1) / G_BM, n_tiles = (N + G_BN - 1) / G_BN;
-  const int num_tiles = m_tiles * n_tiles;
-  const int kb_per_seg = K / G_BK;
-  const int num_kb = kb_per_seg * seg.nseg;
+  const int n_tiles = (N + G_BN - 1) / G_BN;
+  const int m_blk = blockIdx.x / n_tiles, n_blk = blockIdx.x % n_tiles;
+  // k-blocks of 128 bytes per operand row: 64 fp16 or 128 e4m3 elements
+  int seg_kb[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) seg_kb[i] = i < seg.nseg ? (seg.f8[i] ? K / (2 * G_BK) : K / G_BK) : 0;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < G_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 256); }
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < G_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-      for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 4); }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
+      tma_prefetch_desc(&tmA);
+      tma_prefetch_desc(&tmB);
       uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      for (int sg = 0; sg < seg.nseg; ++sg) {
+        for (int kb = 0; kb < seg_kb[sg]; ++kb, ++it) {
           const int s = it % G_STAGES;
           const uint32_t ph = (it / G_STAGES) & 1;
           mbar_wait(&empty_bar[s], ph ^ 1);
-          const int sg = kb / kb_per_seg, kk = (kb % kb_per_seg) * G_BK;
+          const int kk = kb * G_BK;   // in fp16 units of the tensor map (an e4m3 block is the same 128 bytes)
           uint8_t* sa = smem + s * G_STAGE_BYTES;
-          uint8_t* sb = sa + G_A_BYTES;
           mbar_expect_tx(&full_bar[s], G_STAGE_BYTES);
           tma_load_2d(sa, &tmA, &full_bar[s], seg.a_off[sg] + kk, m_blk * G_BM);
-          tma_load_2d(sb, &tmB, &full_bar[s], seg.b_off[sg] + kk, n_blk * G_BN);
+          tma_load_2d(sa + G_A_BYTES, &tmB, &full_bar[s], seg.b_off[sg] + kk, n_blk * G_BN);
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      uint32_t it = 0, tl = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tl) {
-        // narrow problems (N < 256, e.g. 64-channel convolutions) issue a narrower UMMA instead of multiplying zero padding
-        const int n_rem = N - (tile % n_tiles) * G_BN;
-        const int mma_n = n_rem >= G_BN ? G_BN : ((n_rem + 15) / 16) * 16;
-        const uint32_t idesc = make_idesc_f16(G_BM, mma_n, ep.is_bf16);
-        const int acc = tl & 1;
-        const uint32_t aph = (tl >> 1) & 1;
-        mbar_wait(&tempty_bar[acc], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * G_BN);
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % G_STAGES;
-          const uint32_t ph = (it / G_STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * G_STAGE_BYTES);
-          const uint64_t adesc = make_smem_desc_sw128(sa);
-          const uint64_t bdesc = make_smem_desc_sw128(sa + G_A_BYTES);
+    return;
+  }
+
+  // -------------------------------------------------------------- consumers: warpgroup g owns rows [64 g, 64 g + 64)
+  const int g = warp >> 2, w = warp & 3;
+  float acc[64];
+  float acc8[64];   // e4m3 segments (dead when !F8)
 #pragma unroll
-          for (int k = 0; k < G_BK / 16; ++k) {
-            // advance 16 halves = 32 B inside the 128 B swizzle atom: +2 in the (addr >> 4) field
-            umma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tfull_bar[acc]);
+  for (int i = 0; i < 64; ++i) acc[i] = acc8[i] = 0.f;
+  uint32_t it = 0;
+  int prev_s = -1;
+  for (int sg = 0; sg < seg.nseg; ++sg) {
+    const bool f8 = F8 && seg.f8[sg] != 0;
+    for (int kb = 0; kb < seg_kb[sg]; ++kb, ++it) {
+      const int s = it % G_STAGES;
+      mbar_wait(&full_bar[s], (it / G_STAGES) & 1);
+      const uint32_t sa = smem_u32(smem + s * G_STAGE_BYTES);
+      const uint64_t adesc = make_smem_desc_sw128(sa + g * 64 * 128);
+      const uint64_t bdesc = make_smem_desc_sw128(sa + G_A_BYTES);
+      wgmma_fence();
+      if (f8) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n128k32_e4m3(acc8, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
+      } else if (ep.is_bf16) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n128k16_bf16(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n128k16_f16(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
       }
-    }
-  } else {
-    // ------------------------------------------------------------ epilogue (warps 2..5 -> TMEM lane quarters 2,3,0,1)
-    const int q = warp & 3;
-    uint32_t tl = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tl) {
-      const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-      const int acc = tl & 1;
-      const uint32_t aph = (tl >> 1) & 1;
-      mbar_wait(&tfull_bar[acc], aph);
-      tc_fence_after();
-      const int m = m_blk * G_BM + q * 32 + lane;
-      const bool row_ok = m < M;
-      long long drow = m;
-      if (ep.rowmap && row_ok) drow = ep.rowmap[m];
-      const bool store_ok = row_ok && drow >= 0;
-#pragma unroll 1
-      for (int ch = 0; ch < G_BN / 32; ++ch) {
-        uint32_t r[32];
-        __syncwarp();
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * G_BN + ch * 32), r);
-        tmem_ld_wait();
-        const int n0 = n_blk * G_BN + ch * 32;
-        if (n0 >= N) continue;  // warp-uniform
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        if (ep.bias) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += __ldg(ep.bias + n0 + j);
-        }
-        if (ep.act == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-        } else if (ep.act == 3) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(v[j]);
-        }
-        if (!store_ok) {
-          // nothing to write for this row (tail of M, or a padding row dropped by rowmap)
-        } else if (ep.out32) {
-          float* o = ep.out32 + (size_t)drow * ep.ldc + n0;
-          if (ep.resid) {
-            const long long rrow = ep.resid_mod > 0 ? (drow % ep.resid_mod) : drow;
-            const float* rs = ep.resid + (size_t)rrow * ep.ldc + n0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 t = *reinterpret_cast<const float4*>(rs + j);
-              v[j] += t.x; v[j + 1] += t.y; v[j + 2] += t.z; v[j + 3] += t.w;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(o + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        } else {
-          __half* o = ep.out16 + (size_t)drow * ep.ldc + n0;
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (ep.is_bf16) {
-              __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-              hi[j] = *reinterpret_cast<uint32_t*>(&h);
-              lo[j] = 0;
-            } else {
-              __half2 h = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
-              hi[j] = *reinterpret_cast<uint32_t*>(&h);
-              float2 hf = __half22float2(h);
-              __half2 l = __floats2half2_rn(v[2 * j] - hf.x, v[2 * j + 1] - hf.y);
-              lo[j] = *reinterpret_cast<uint32_t*>(&l);
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(o + 2 * j) = make_uint4(hi[j], hi[j + 1], hi[j + 2], hi[j + 3]);
-          if (ep.split_off > 0) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 4)
-              *reinterpret_cast<uint4*>(o + ep.split_off + 2 * j) = make_uint4(lo[j], lo[j + 1], lo[j + 2], lo[j + 3]);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+      wgmma_commit();
+      wgmma_wait<1>();   // the previous k-block's wgmmas have finished reading their stage
+      if (prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+      prev_s = s;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  if (F8) wgmma_fence_regs(acc8);
+
+  // -------------------------------------------------------------- epilogue straight from the accumulator registers
+  const float acc_scale = ep.acc_scale ? __ldg(ep.acc_scale) : 1.0f;
+  const int c2 = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m_blk * G_BM + g * 64 + w * 16 + (lane >> 2) + 8 * h;
+    if (m >= M) continue;
+    long long drow = m;
+    if (ep.rowmap) drow = ep.rowmap[m];
+    if (drow < 0) continue;   // a padding row dropped by rowmap
+#pragma unroll
+    for (int i = 0; i < G_BN / 8; ++i) {
+      const int n = n_blk * G_BN + 8 * i + c2;
+      if (n >= N) continue;   // N % 8 == 0: the pair is in or out together
+      float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+      if (F8) { v0 += acc8[4 * i + 2 * h]; v1 += acc8[4 * i + 2 * h + 1]; }
+      v0 *= acc_scale; v1 *= acc_scale;
+      if (ep.bias) { v0 += __ldg(ep.bias + n); v1 += __ldg(ep.bias + n + 1); }
+      if (ep.act == 1) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+      else if (ep.act == 3) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
+      if (ep.out32) {
+        float* o = ep.out32 + (size_t)drow * ep.ldc + n;
+        if (ep.resid) {
+          const long long rrow = ep.resid_mod > 0 ? (drow % ep.resid_mod) : drow;
+          const float2 t = *reinterpret_cast<const float2*>(ep.resid + (size_t)rrow * ep.ldc + n);
+          v0 += t.x; v1 += t.y;
+        }
+        *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+      } else if (ep.is_bf16) {
+        *reinterpret_cast<__nv_bfloat162*>(ep.out16 + (size_t)drow * ep.ldc + n) = __floats2bfloat162_rn(v0, v1);
+      } else {
+        __half* o = ep.out16 + (size_t)drow * ep.ldc + n;
+        const __half2 hv = __floats2half2_rn(v0, v1);
+        *reinterpret_cast<__half2*>(o) = hv;
+        const float2 hf = __half22float2(hv);
+        if (ep.split_off > 0 && ep.out_f8) {
+          // fp8 correction operands of the next GEMM (tc_api.cuh): remainder * 2^12 and value * 2^-3 as e4m3 bytes
+          uint8_t* ob = reinterpret_cast<uint8_t*>(ep.out16 + (size_t)drow * ep.ldc + ep.split_off) + n;
+          uint16_t l8, h8;
+          asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(l8) : "f"((v1 - hf.y) * F8_LO_SCALE), "f"((v0 - hf.x) * F8_LO_SCALE));
+          asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h8) : "f"(v1 * F8_HI_SCALE), "f"(v0 * F8_HI_SCALE));
+          *reinterpret_cast<uint16_t*>(ob) = l8;
+          *reinterpret_cast<uint16_t*>(ob + ep.split_off) = h8;
+        } else if (ep.split_off > 0) {
+          *reinterpret_cast<__half2*>(o + ep.split_off) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+        }
+      }
+    }
   }
 }
+
+// the shapes on which precision 6 runs its correction passes in e4m3 (the ViT's linear layers; other GEMMs keep three fp16
+// passes): whole 128-element e4m3 k-blocks
+bool gemm_f8c_applicable(int M, int N, int K) { return M >= 256 && N % 256 == 0 && K % (2 * G_BK) == 0; }
 
 int gemm_tc(Ctx* c, cudaStream_t st, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const GemmSeg& seg,
             const GemmEpi& ep) {
@@ -213,20 +174,22 @@ int gemm_tc(Ctx* c, cudaStream_t st, const void* A, int lda, const void* B, int 
   SAMPT_CHECK(seg.nseg >= 1 && seg.nseg <= 3, "gemm_tc: nseg out of range");
   SAMPT_CHECK((ep.out16 != nullptr) != (ep.out32 != nullptr), "gemm_tc: exactly one of out16/out32 must be set");
   SAMPT_CHECK(ep.ldc % 8 == 0, "gemm_tc: ldc must be a multiple of 8");
-  if (gemm_tc2_applicable(M, N, K, ep)) {
-    SAMPT_CHECK(!(seg.f8[0] | seg.f8[1] | seg.f8[2]) || K % 128 == 0, "gemm_tc: e4m3 segments need K %% 128 == 0 (K = %d)", K);
-    return gemm_tc2(c, st, A, lda, B, ldb, M, N, K, seg, ep);
-  }
-  SAMPT_CHECK(!(seg.f8[0] | seg.f8[1] | seg.f8[2]) && !ep.out_f8 && ep.acc_scale == nullptr,
-              "gemm_tc: the fp8-corrected GEMM runs on the CTA-pair kernel only (M >= 256, N %% 256 == 0, K %% 128 == 0)");
-  SAMPT_TRY(ensure_func_smem(c, "gemm_tc_kernel", gemm_tc_kernel, G_SMEM_BYTES));
+  const bool f8 = (seg.f8[0] | seg.f8[1] | seg.f8[2]) != 0;
+  SAMPT_CHECK(!f8 || K % (2 * G_BK) == 0, "gemm_tc: e4m3 segments need K %% 128 == 0 (K = %d)", K);
+  SAMPT_CHECK(!f8 || !ep.is_bf16, "gemm_tc: e4m3 segments go with fp16 operands");
   CUtensorMap tmA, tmB;
   // the A/B matrices may carry several K segments side by side (hi | lo): inner extent = lda / ldb
   SAMPT_TRY(make_tmap_2d_f16(&tmA, A, (uint64_t)lda, (uint64_t)M, (uint64_t)lda * 2, G_BK, G_BM));
   SAMPT_TRY(make_tmap_2d_f16(&tmB, B, (uint64_t)ldb, (uint64_t)N, (uint64_t)ldb * 2, G_BK, G_BN));
   const int m_tiles = (M + G_BM - 1) / G_BM, n_tiles = (N + G_BN - 1) / G_BN;
-  int grid = std::min(m_tiles * n_tiles, c->num_sms);
-  gemm_tc_kernel<<<grid, G_THREADS, G_SMEM_BYTES, st>>>(tmA, tmB, M, N, K, seg, ep);
+  const int grid = m_tiles * n_tiles;
+  if (f8) {
+    SAMPT_TRY(ensure_func_smem(c, "gemm_tc_kernel<f8>", gemm_tc_kernel<true>, G_SMEM_BYTES));
+    gemm_tc_kernel<true><<<grid, G_THREADS, G_SMEM_BYTES, st>>>(tmA, tmB, M, N, K, seg, ep);
+  } else {
+    SAMPT_TRY(ensure_func_smem(c, "gemm_tc_kernel", gemm_tc_kernel<false>, G_SMEM_BYTES));
+    gemm_tc_kernel<false><<<grid, G_THREADS, G_SMEM_BYTES, st>>>(tmA, tmB, M, N, K, seg, ep);
+  }
   c->launches++;
   SAMPT_LAUNCH_CHECK();
   return 0;

@@ -33,7 +33,7 @@ static bool fnet_uses_tc(const Ctx* c, const std::string& prefix) {
 
 static int conv_by_name(Ctx* c, cudaStream_t st, const std::string& name, const Act& in, Act* out, int R, int stride, int pad) {
   if (c->fnet_im2col != nullptr) {
-    // implicit-GEMM on tcgen05: A = im2col(in) as fp16 hi|lo, B = weights hi|lo, 3 split passes (~fp32), fp32 NHWC output
+    // implicit-GEMM on tensor cores: A = im2col(in) as fp16 hi|lo, B = weights hi|lo, 3 split passes (~fp32), fp32 NHWC output
     const __half* w16; const float* b;
     SAMPT_TRY(get_f16(c, c->fnet_prefix + name + ".w16", &w16));
     SAMPT_TRY(get_f32(c, c->fnet_prefix + name + ".bias", &b));

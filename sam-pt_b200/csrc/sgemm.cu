@@ -2,7 +2,7 @@
 //
 // Used where the reference's numerics must be kept at float32 (PIPS MLP-Mixer: the 1e-3 px tolerance with a
 // 6-iteration feedback loop, SURVEY §7 "parity under chaos"; SAM prompt/mask decoder: 12 mask->box->mask
-// refinement iterations).  Tensor-core GEMMs (tcgen05) live in gemm_tc.cu and serve the ViT encoder.
+// refinement iterations).  Tensor-core GEMMs (wgmma) live in gemm_tc.cu and serve the ViT encoder.
 #include <cooperative_groups.h>
 #include <cstdlib>
 
@@ -342,7 +342,7 @@ int sgemm_nt_skip(Ctx* c, cudaStream_t st, const float* X, int ldx, const float*
     SAMPT_CHECK(rc != 2, "sgemm_nt: cluster launch of the skinny kernel failed (%s)", cudaGetErrorString(cudaGetLastError()));
     if (rc == 1) SAMPT_TRY((launch_pipe<64, 16, 4, 1, 4>(st, X, ldx, W, ldw, bias, residual, ldr, Y, ldy, M, N, K, act, skip)));
   } else {
-    // tile choice: the largest tile that still yields enough CTAs for 148 SMs
+    // tile choice: the largest tile that still yields enough CTAs for 132 SMs
     const long long t128 = (long long)cdiv(M, 128) * cdiv(N, 64), t64 = (long long)cdiv(M, 64) * cdiv(N, 64);
     if (t128 >= 2 * c->num_sms) {
       SAMPT_TRY((launch_pipe<128, 64, 8, 4, 3>(st, X, ldx, W, ldw, bias, residual, ldr, Y, ldy, M, N, K, act, skip)));

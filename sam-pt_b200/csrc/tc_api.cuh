@@ -24,7 +24,7 @@ struct GemmEpi {
 
 // K-loop segments for split precision: segment i multiplies A[:, a_off[i] : a_off[i]+K] with B[:, b_off[i] : b_off[i]+K]
 // (offsets in fp16 units).  f8[i] != 0: the segment's operands are e4m3 BYTES (K of them = K/2 fp16 units starting at the
-// offset), multiplied with tcgen05.mma.kind::f8f6f4 at twice the fp16 rate into the same fp32 accumulator (gemm_tc2 only).
+// offset), multiplied with wgmma e4m3 at twice the fp16 rate into a second fp32 accumulator that the epilogue adds.
 struct GemmSeg { int nseg; int a_off[3]; int b_off[3]; int f8[3]; };
 
 // fp8-corrected split GEMM ("precision 6"), operand rows of 2K fp16 units:
@@ -44,20 +44,10 @@ inline GemmSeg make_seg_f8(int K) {
 
 int gemm_tc(Ctx* c, cudaStream_t st, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const GemmSeg& seg,
             const GemmEpi& ep);
-
-// out_f8 (only where attn_ws_applicable): the output row carries the fp8 correction operands of the proj GEMM instead of the fp16 remainder
-int attn_tc(Ctx* c, cudaStream_t st, const __half* Qx, const __half* Kx, const __half* Vt, int BH, int Lq, int Lk, int Lkp,
-            int DK, int HD, int NT, int nheads, __half* out, int ld_out, int split_off, int out_f8 = 0);
-
-// CTA-pair (cta_group::2) variant of gemm_tc (gemm_tc2.cu); on unless SAMPT_GEMM_2CTA=0
-bool gemm_tc2_applicable(int M, int N, int K, const GemmEpi& ep);
 bool gemm_f8c_applicable(int M, int N, int K);   // shapes the fp8-corrected segments (GemmSeg::f8) run on
-int gemm_tc2(Ctx* c, cudaStream_t st, const void* A, int lda, const void* B, int ldb, int M, int N, int K, const GemmSeg& seg,
-             const GemmEpi& ep);
 
-// round-2 kernel: two softmax warpgroups, P in tensor memory (TS MMA), persistent (attn_ws.cu); on unless SAMPT_ATTN_WS=0
-bool attn_ws_applicable(int Lk, int DK, int HD, int NT);
-int attn_ws(Ctx* c, cudaStream_t st, const __half* Qx, const __half* Kx, const __half* Vt, int BH, int Lq, int Lk, int Lkp, int DK,
-            int HD, int NT, int nheads, __half* out, int ld_out, int split_off, int out_f8 = 0);
+// out_f8: the output row carries the fp8 correction operands of the proj GEMM instead of the fp16 remainder
+int attn_tc(Ctx* c, cudaStream_t st, const __half* Qx, const __half* Kx, const __half* Vt, int BH, int Lq, int Lk, int Lkp,
+            int DK, int HD, int nheads, __half* out, int ld_out, int split_off, int out_f8 = 0);
 
 }  // namespace sampt

@@ -1,7 +1,7 @@
-// Host-side orchestration of SAM's ImageEncoderViT on the B200 (C++; one stream).
+// Host-side orchestration of SAM's ImageEncoderViT (C++; one stream).
 // Upstream: segment_anything/modeling/image_encoder.py (un-vendored; SURVEY Appendix B.1); reference call site
 // sam_pt/modeling/sam_pt.py:849 (SamPredictor.set_image).  Frames are batched (B) so every GEMM has M = B*4096 (or
-// B*4900 window-partitioned rows) and fills 148 SMs.
+// B*4900 window-partitioned rows) and fills every SM.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -111,8 +111,8 @@ static int vit_forward(Ctx* c, cudaStream_t st, const uint8_t* img, const float*
   // precision 5: like 3, but the attention OUTPUT is carried as fp16 hi|lo and the proj GEMM runs all three passes -- the
   // attention kernel accumulates O in fp32, so this removes the 2^-11 rounding of proj's input; qkv stays at two passes (its
   // output is rounded to fp16 for the attention operands whatever the GEMM does).
-  // precision 6: like 4 (every product to ~2^-22), but the two CORRECTION passes of the qkv / lin1 / lin2 GEMMs run in e4m3 on
-  // tcgen05.mma.kind::f8f6f4 at twice the fp16 rate: A_lo.B_hi and A_hi.B_lo are 2^-12 of the result, so the 2^-5 relative
+  // precision 6: like 4 (every product to ~2^-22), but the two CORRECTION passes of the qkv / proj / lin1 / lin2 GEMMs run in
+  // e4m3 wgmma at twice the fp16 rate: A_lo.B_hi and A_hi.B_lo are 2^-12 of the result, so the 2^-5 relative
   // rounding of their fp8 operands leaves a 2^-17 residual (tc_api.cuh: make_seg_f8).  2 fp16-pass equivalents instead of 3.
   const bool f8c = precision == 6;
   const int p_qkv = (precision == 3 || precision == 5) ? 2 : (precision >= 4 ? 3 : precision);
@@ -249,10 +249,9 @@ static int vit_forward(Ctx* c, cudaStream_t st, const uint8_t* img, const float*
     const int nwb = is_global ? B : (live_only ? B * nLW : B * nW * nW);
     const int DK = is_global ? DKg : DKw;
     const int Lkp = is_global ? GG : Lkpw;
-    const int NT = is_global ? 128 : (((Lw + 15) / 16) * 16 <= 256 ? ((Lw + 15) / 16) * 16 : 128);
-    // which GEMMs of this block take the fp8-corrected form (shape gate of the CTA-pair kernel; else three fp16 passes)
+    // which GEMMs of this block take the fp8-corrected form (gemm_f8c_applicable; else three fp16 passes)
     const bool f8_qkv = f8c && gemm_f8c_applicable(Mrows, 3 * D, D);
-    const bool f8_proj = f8c && gemm_f8c_applicable(Mrows, D, D) && attn_ws_applicable(L, DK, HD, NT);   // (attn_ws writes the layout)
+    const bool f8_proj = f8c && gemm_f8c_applicable(Mrows, D, D);
     const bool f8_l1 = f8c && gemm_f8c_applicable(Mmlp, 4 * D, D);
     const bool f8_l2 = f8c && gemm_f8c_applicable(Mmlp, D, 4 * D);
     // LN1 (+ window partition with zero padding)
@@ -271,7 +270,7 @@ static int vit_forward(Ctx* c, cudaStream_t st, const uint8_t* img, const float*
     }
     // attention
     SAMPT_TRY(attn_prep(c, st, qkv, 3 * D, rph, rpw, Qx, Kx, Vt, nwb, d.nheads, S, Lkp, DK, D, HD, 1.0f / sqrtf((float)HD)));
-    SAMPT_TRY(attn_tc(c, st, Qx, Kx, Vt, nwb * d.nheads, L, L, Lkp, DK, HD, NT, d.nheads, att, D * asp, (asp == 2 && p_proj == 3) ? D : 0,
+    SAMPT_TRY(attn_tc(c, st, Qx, Kx, Vt, nwb * d.nheads, L, L, Lkp, DK, HD, d.nheads, att, D * asp, (asp == 2 && p_proj == 3) ? D : 0,
                       f8_proj));
     // x = x + proj(attn)   (window un-partition via the row map; padding rows are dropped)
     {

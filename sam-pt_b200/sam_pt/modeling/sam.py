@@ -36,5 +36,5 @@ def __getattr__(name):
         globals()["SamHQHydra"] = SamHQHydra
         return SamHQHydra
     if name == "MobileSamHydra":
-        raise ImportError("MobileSAM is outside the B200 hot-path scope (SURVEY §2 row 2)")
+        raise ImportError("MobileSAM is outside the H100 hot-path scope (SURVEY §2 row 2)")
     raise AttributeError(name)

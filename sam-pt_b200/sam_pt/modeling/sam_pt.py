@@ -2,7 +2,7 @@
 contract and output dict.  The per-frame work is re-organised for the GPU:
 
 * the clip is uploaded once (uint8), the tracker consumes it on the device;
-* SAM's encoder runs on batches of frames (tcgen05 GEMMs need M = B*4096 rows to fill 148 SMs);
+* SAM's encoder runs on batches of frames (tensor-core GEMMs need M = B*4096 rows to fill 132 SMs);
 * `predict_mask`'s 1-2 + <=12 `predict_torch` calls per (frame, mask) are ONE native call with the `area < 2` break test
   evaluated on the device (the reference synchronises ~6x per refinement iteration, sam_pt.py:811-820);
 * one device->host copy per clip (trajectories + visibilities, a few KB) replaces the per-frame copies; the host then

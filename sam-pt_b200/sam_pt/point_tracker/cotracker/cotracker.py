@@ -76,7 +76,7 @@ class CoTracker(nn.Module):
     def __init__(self, S=8, stride=4, add_space_attn=True, num_heads=8, hidden_size=384, space_depth=6, time_depth=6):
         super().__init__()
         if (S, stride, add_space_attn, num_heads, hidden_size) != (8, 4, True, 8, 384):
-            raise NotImplementedError("the B200 CoTracker path is built for cotracker_stride_4_wind_8 "
+            raise NotImplementedError("the H100 CoTracker path is built for cotracker_stride_4_wind_8 "
                                       "(configs/model/point_tracker/cotracker.yaml:2)")
         self.S, self.stride = S, stride
         self.latent_dim = LATENT
@@ -107,7 +107,7 @@ class CoTracker(nn.Module):
                         ctx.set_tensor(f"cot.{k[:-len('.weight')]}.w16", torch.cat([hi, lo], dim=1).contiguous())
                 else:
                     ctx.set_tensor(f"cot.{k}", v.contiguous())
-                    # UpdateFormer linear layers also as fp16 hi | lo [N, 2K] for the three-pass tcgen05 GEMM (csrc/cotracker.cu: cot_tcg)
+                    # UpdateFormer linear layers also as fp16 hi | lo [N, 2K] for the three-pass tensor-core GEMM (csrc/cotracker.cu: cot_tcg)
                     if k.startswith("updateformer.") and k.endswith(".weight") and ("_blocks." in k) and v.dim() == 2:
                         hi = v.half()
                         lo = (v - hi.float()).half()
@@ -210,7 +210,7 @@ class CoTracker(nn.Module):
     def forward(self, rgbs, queries, iters=4, feat_init=None, is_train=False):
         """Upstream signature; rgbs (1,T,3,H,W) float 0..255, queries (1,N,3) -> (traj (1,T,N,2), feat_init, vis (1,T,N), None)."""
         if feat_init is not None or is_train:
-            raise NotImplementedError("B200 CoTracker covers inference with feat_init=None")
+            raise NotImplementedError("H100 CoTracker covers inference with feat_init=None")
         if rgbs.shape[0] != 1:
             raise NotImplementedError("batch size 1 (the SAM-PT hot path tracks one clip at a time)")
         T = rgbs.shape[1]

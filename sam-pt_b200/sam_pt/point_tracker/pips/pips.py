@@ -62,7 +62,7 @@ class Pips(nn.Module):
         self.corr_radius = 3
         build_param_tree(self, _pips_shapes(S), seed=486124)
         self._registered_on = None
-        # BasicEncoder convolutions as im2col + tcgen05 GEMM with 3-pass fp16 split (~fp32); "0" = strict fp32 CUDA-core path
+        # BasicEncoder convolutions as im2col + tensor-core GEMM with 3-pass fp16 split (~fp32); "0" = strict fp32 CUDA-core path
         self.fnet_on_tensor_cores = os.environ.get("SAMPT_PIPS_TC", "1") != "0"
 
     # ------------------------------------------------------------------ weights -> kernel-native layouts
@@ -81,7 +81,7 @@ class Pips(nn.Module):
                 if k.startswith("fnet.") and k.endswith(".weight") and v.dim() == 4:
                     ctx.set_tensor(f"pips.{k}_rsck", v.permute(2, 3, 1, 0).contiguous())
                     if self.fnet_on_tensor_cores:
-                        # tcgen05 path: [Cout, 2*Kp] fp16 hi|lo, k = (r*S + s)*Cin + ci, K zero-padded to a multiple of 64
+                        # tensor-core path: [Cout, 2*Kp] fp16 hi|lo, k = (r*S + s)*Cin + ci, K zero-padded to a multiple of 64
                         w = v.permute(0, 2, 3, 1).reshape(v.shape[0], -1)
                         kp = -(-w.shape[1] // 64) * 64
                         wp = torch.zeros((w.shape[0], kp), device=w.device)
@@ -104,7 +104,7 @@ class Pips(nn.Module):
         """(n,3,H,W) uint8 -> channels-last encoder features (n,H/4,W/4,128) fp32 (BasicEncoder, once per frame)."""
         assert frames_u8.dtype == torch.uint8 and frames_u8.is_cuda
         if self.stride != 4:
-            raise NotImplementedError("the B200 PIPS path is built for stride 4 (configs/model/point_tracker/pips.yaml:3)")
+            raise NotImplementedError("the H100 PIPS path is built for stride 4 (configs/model/point_tracker/pips.yaml:3)")
         ctx = self.native_context()
         n, _, H, W = frames_u8.shape
         fm = torch.empty((n, H // 4, W // 4, LATENT), device=frames_u8.device, dtype=torch.float32)
@@ -152,7 +152,7 @@ class Pips(nn.Module):
         estimate (:479-480,571-572); vis_e (1,S,N) raw logits (:568); [ffeat (1,N,128) if return_feat (:617-618);] losses=None).
         One native call (`sampt_pips_window`)."""
         if trajs_g is not None or is_train or self.training or (sw is not None and getattr(sw, "save_this", False)):
-            raise NotImplementedError("B200 Pips.forward covers inference (no losses / training / summary writer)")
+            raise NotImplementedError("H100 Pips.forward covers inference (no losses / training / summary writer)")
         B, N, D = xys.shape
         assert D == 2
         if B != 1:

@@ -1,4 +1,4 @@
-"""In-tree build of libsampt_b200.so with plain nvcc for sm_100a (no torch C++ extension: the boundary is a C ABI)."""
+"""In-tree build of libsampt_b200.so with plain nvcc for sm_90a (no torch C++ extension: the boundary is a C ABI)."""
 from __future__ import annotations
 
 import os
@@ -11,23 +11,35 @@ CSRC = os.path.join(PKG_ROOT, "csrc")
 LIB_DIR = os.path.join(PKG_ROOT, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libsampt_b200.so")
 
-# sm_100a only; no --use_fast_math: sinf/cosf/expf/erff must stay the accurate versions (flow embeddings reach ~1e5 rad)
-NVCC_COMPILE_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
+# sm_90a only (wgmma / TMA); no --use_fast_math: sinf/cosf/expf/erff must stay the accurate versions (flow embeddings reach ~1e5 rad)
+NVCC_COMPILE_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found (needed to build libsampt_b200.so for sm_100a)")
+    raise RuntimeError("nvcc not found (needed to build libsampt_b200.so for sm_90a)")
 
 
 def sources():
     return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
 
 
+OBJ_DIR = os.path.join(PKG_ROOT, "build")
+FLAGS_STAMP = os.path.join(OBJ_DIR, "nvcc_flags.txt")   # objects built with other flags (another architecture) are rebuilt
+
+
+def _flags_changed() -> bool:
+    try:
+        with open(FLAGS_STAMP) as f:
+            return f.read() != " ".join(NVCC_COMPILE_FLAGS)
+    except OSError:
+        return True
+
+
 def is_stale() -> bool:
-    if not os.path.exists(LIB_PATH):
+    if not os.path.exists(LIB_PATH) or _flags_changed():
         return True
     t = os.path.getmtime(LIB_PATH)
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [
@@ -40,8 +52,9 @@ def build_native(force: bool = False, verbose: bool = False) -> str:
     if not force and not is_stale():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
-    objdir = os.path.join(PKG_ROOT, "build")
+    objdir = OBJ_DIR
     os.makedirs(objdir, exist_ok=True)
+    force = force or _flags_changed()
     nvcc = _nvcc()
     procs = []
     objs = []
@@ -61,10 +74,12 @@ def build_native(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
         if verbose and out:
             print(out, file=sys.stderr)
-    link = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH] + objs + ["-lcudart"]
+    link = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB_PATH] + objs + ["-lcudart"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")
+    with open(FLAGS_STAMP, "w") as f:
+        f.write(" ".join(NVCC_COMPILE_FLAGS))
     return LIB_PATH
 
 

@@ -52,7 +52,7 @@ class Context:
 
     def __init__(self, device: torch.device, workspace_bytes: int = 8 << 30):
         if not torch.cuda.is_available():
-            raise RuntimeError("libsampt_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("libsampt_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device(device)
         self._h = c_void_p()
         with torch.cuda.device(self.device):
@@ -136,7 +136,7 @@ def get_context(device) -> Context:
     """One shared context per device (weights of SAM and of the tracker are registered under distinct prefixes)."""
     device = torch.device(device)
     if device.type != "cuda":
-        raise RuntimeError(f"the SAM-PT B200 path runs on CUDA only (got device {device}); there is no CPU fallback")
+        raise RuntimeError(f"the SAM-PT H100 path runs on CUDA only (got device {device}); there is no CPU fallback")
     idx = device.index if device.index is not None else torch.cuda.current_device()
     if idx not in _contexts:
         _contexts[idx] = Context(torch.device("cuda", idx))

@@ -6,7 +6,7 @@ of T frames every rank owns exactly T frames (round 1 gave rank r frames r, r+G,
 G=8, a 0.89 ceiling on the 8-GPU efficiency).
 
 The one exchange step of the path is an all-gather of per-frame tracker feature maps; this module holds the index arithmetic +
-the collective wrappers so they can be tested with gloo on CPU (world_size 2 / 4) and run with NCCL on the B200s.
+the collective wrappers so they can be tested with gloo on CPU (world_size 2 / 4) and run with NCCL on the H100s.
 """
 from __future__ import annotations
 

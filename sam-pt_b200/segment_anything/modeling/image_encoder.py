@@ -1,6 +1,6 @@
 """`ImageEncoderViT` with upstream constructor kwargs / state-dict keys (segment_anything/modeling/image_encoder.py @ aac76a1;
 kwargs per /root/reference/configs/model/sam/image_encoder/vit_base.yaml:1-16) executing in libsampt_b200:
-tcgen05 GEMMs + fused attention (csrc/gemm_tc.cu, attn_tc.cu, vit_kernels.cu, vit_pipeline.cu)."""
+tensor-core GEMMs + fused attention (csrc/gemm_tc.cu, attn_tc.cu, vit_kernels.cu, vit_pipeline.cu)."""
 from __future__ import annotations
 
 import math
@@ -14,17 +14,17 @@ from torch import nn
 from sampt_b200 import native
 from sampt_b200.param_tree import build_param_tree
 
-# GEMM accuracy dial (DESIGN.md "precision"): operands are carried as fp16 hi | lo (lo = fp16(x - hi)) and the tcgen05 K loop runs
-# over up to three segments A_hi.B_hi + A_lo.B_hi + A_hi.B_lo into one fp32 TMEM accumulator.
+# GEMM accuracy dial (DESIGN.md "precision"): operands are carried as fp16 hi | lo (lo = fp16(x - hi)) and the tensor-core K loop runs
+# over up to three segments A_hi.B_hi + A_lo.B_hi + A_hi.B_lo into one fp32 register accumulator.
 #   1 = fp16 x fp16, one pass          2 = weights hi|lo, two passes          3 = MLP three passes, qkv / proj two
 #   5 = MLP + proj three passes (attention output kept as hi|lo), qkv two     4 = three passes everywhere (~fp32 products)
-#   6 = like 4, but the two correction segments of the qkv / proj / lin1 / lin2 GEMMs are e4m3 operands on kind::f8f6f4 at twice
-#       the fp16 rate (they are 2^-12 of the result, e4m3's 2^-5 rounding leaves 2^-17): 2 fp16-pass equivalents instead of 3
-# Measured on the B200 against the FULL BASELINE clips (tests/test_gpu_full_configs.py: 50 frames of C2, 50 of C3, 8 of the C5
-# slice; bar: per-frame IoU >= 0.999), min IoU C2 / C3 / C5s:  3: 0.99878 / - / 0.99873 (fails);  5: 0.99911 / - / 0.99951 (one
-# frame of C2 within 1e-4 of the bar);  4: 0.99979 / 0.99971 / 0.99961;  6: 0.99978 / 0.99973 / 0.99966 at +16 % frames/s over 4.
-# With random weights the mask logits are noise-like and the 12-step box refinement amplifies a 1-pixel box change into ~1e-3
-# IoU, so only 4 and 6 clear the bar with margin; 6 is the default.
+#   6 = like 4, but the two correction segments of the qkv / proj / lin1 / lin2 GEMMs are e4m3 operands (e4m3 wgmma at twice
+#       the fp16 rate, accumulated apart from the fp16 pass): they are 2^-12 of the result, e4m3's 2^-5 rounding leaves 2^-17,
+#       so 2 fp16-pass equivalents instead of 3
+# Measured at 6 on one H100 (400 W) against the FULL BASELINE clips (tests/test_gpu_full_configs.py: 50 frames of C2, 50 of C3,
+# 8 of the C5 slice; bar: per-frame IoU >= 0.999), min IoU C2 / C3 / C5s: 0.99976 / 0.99971 / 0.99963.  With random weights the
+# mask logits are noise-like and the 12-step box refinement amplifies a 1-pixel box change into ~1e-3 IoU, so settings that drop a
+# correction term (2, 3, 5) sit close to or below the bar; 6 is the default.
 DEFAULT_PRECISION = int(os.environ.get("SAMPT_VIT_PRECISION", "6"))
 
 
@@ -36,7 +36,7 @@ class ImageEncoderViT(nn.Module):
                  global_attn_indexes: Tuple[int, ...] = ()) -> None:
         super().__init__()
         if not (use_abs_pos and use_rel_pos and qkv_bias and in_chans == 3 and int(mlp_ratio) == 4):
-            raise NotImplementedError("the B200 encoder implements SAM's configuration: abs+rel pos, qkv bias, mlp_ratio 4")
+            raise NotImplementedError("the H100 encoder implements SAM's configuration: abs+rel pos, qkv bias, mlp_ratio 4")
         self.img_size, self.patch_size, self.embed_dim, self.depth = img_size, patch_size, embed_dim, depth
         self.num_heads, self.out_chans, self.window_size = num_heads, out_chans, window_size
         self.global_attn_indexes = tuple(int(i) for i in global_attn_indexes)

@@ -10,7 +10,7 @@ class MaskDecoder(nn.Module):
                  iou_head_depth: int = 3, iou_head_hidden_dim: int = 256) -> None:
         super().__init__()
         if (transformer_dim, num_multimask_outputs, iou_head_depth, iou_head_hidden_dim) != (256, 3, 3, 256):
-            raise NotImplementedError("the B200 mask decoder is built for SAM: dim 256, 3 multimask outputs, 3-layer heads")
+            raise NotImplementedError("the H100 mask decoder is built for SAM: dim 256, 3 multimask outputs, 3-layer heads")
         self.transformer_dim = transformer_dim
         self.transformer = transformer
         self.num_multimask_outputs = num_multimask_outputs

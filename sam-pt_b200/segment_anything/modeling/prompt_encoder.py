@@ -15,7 +15,7 @@ class PromptEncoder(nn.Module):
                  mask_in_chans: int, activation=nn.GELU) -> None:
         super().__init__()
         if embed_dim != 256 or mask_in_chans != 16:
-            raise NotImplementedError("the B200 prompt encoder is built for embed_dim=256, mask_in_chans=16 (SAM)")
+            raise NotImplementedError("the H100 prompt encoder is built for embed_dim=256, mask_in_chans=16 (SAM)")
         self.embed_dim = embed_dim
         self.image_embedding_size = tuple(image_embedding_size)
         self.input_image_size = tuple(input_image_size)

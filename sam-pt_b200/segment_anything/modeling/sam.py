@@ -69,7 +69,7 @@ class Sam(nn.Module):
         ctx.set_tensor("sam.mask_decoder.output_upscaling.0.weight_gemm", w0.permute(2, 3, 1, 0).reshape(-1, w0.shape[0]))
         ctx.set_tensor("sam.mask_decoder.output_upscaling.0.bias4", sd["output_upscaling.0.bias"].float().repeat(4))
 
-        # image-side projections (4096-row operands) run on the tcgen05 GEMM with the 3-pass fp16 hi|lo split (~fp32 products):
+        # image-side projections (4096-row operands) run on the tensor-core GEMM with the 3-pass fp16 hi|lo split (~fp32 products):
         # weights as [N, 2K] = hi | lo
         def w16(wm):
             wm = wm.float()

@@ -10,7 +10,7 @@ class TwoWayTransformer(nn.Module):
                  attention_downsample_rate: int = 2) -> None:
         super().__init__()
         if (depth, embedding_dim, num_heads, mlp_dim, attention_downsample_rate) != (2, 256, 8, 2048, 2):
-            raise NotImplementedError("the B200 mask decoder is built for SAM's two-way transformer: depth 2, dim 256, "
+            raise NotImplementedError("the H100 mask decoder is built for SAM's two-way transformer: depth 2, dim 256, "
                                       "8 heads, mlp 2048, downsample 2")
         self.depth, self.embedding_dim, self.num_heads, self.mlp_dim = depth, embedding_dim, num_heads, mlp_dim
         c, ci = embedding_dim, embedding_dim // attention_downsample_rate

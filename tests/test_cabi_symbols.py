@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds (nvcc cross-compiles sm_100a without a GPU), loads, and exports every symbol that
+"""CPU: the C-ABI library builds (nvcc cross-compiles sm_90a without a GPU), loads, and exports every symbol that
 include/sampt_b200.h declares.  No compute is called."""
 import ctypes
 import os

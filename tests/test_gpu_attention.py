@@ -1,4 +1,4 @@
-"""GPU: tcgen05 flash-attention kernel (pre-extended operands) against a float64 softmax(QK^T)V reference."""
+"""GPU: tensor-core flash-attention kernel (pre-extended operands) against a float64 softmax(QK^T)V reference."""
 from ctypes import c_int
 
 import pytest

@@ -105,7 +105,7 @@ def test_tracker_wrapper_vs_oracle(T):
 
 
 def test_tensor_core_encoder_end_to_end():
-    """default configuration (encoder convolutions on tcgen05 with the 3-pass split): trajectories within 1e-3 px of the oracle."""
+    """default configuration (encoder convolutions on tensor cores with the 3-pass split): trajectories within 1e-3 px of the oracle."""
     from oracle import cotracker_ref as R
     sd = _weights()
     T, H, W = 12, 96, 128

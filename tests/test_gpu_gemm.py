@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMEM/TMA GEMM against a float64 torch reference of the same op (tolerances stated per mode)."""
+"""GPU: the wgmma/TMA GEMM against a float64 torch reference of the same op (tolerances stated per mode)."""
 from ctypes import c_int
 
 import pytest

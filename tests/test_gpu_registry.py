@@ -74,7 +74,7 @@ def test_two_contexts_on_one_device_are_independent():
     gives the same results as the first one, before and after the first one is used again."""
     from sampt_b200 import native
     g = torch.Generator().manual_seed(5)
-    M, N, K = 512, 512, 256          # CTA-pair kernel (dynamic shared memory attribute set per context)
+    M, N, K = 512, 512, 256          # tensor-core GEMM (dynamic shared memory attribute set per context)
     A = torch.randn((M, K), generator=g).half().cuda()
     B = (torch.randn((N, K), generator=g) / K ** 0.5).half().cuda()
     ctx_a = native.get_context("cuda")

@@ -61,7 +61,7 @@ def test_vit_encoder_matches_oracle(vit, precision, tol):
 
 @pytest.mark.parametrize("precision", [4, 6])
 def test_vit_b_precision3_embedding(precision):
-    """ViT-B (every block GEMM on the CTA-pair kernel): three fp16 passes (4) and fp16 + two e4m3 correction passes (6)."""
+    """ViT-B (every block GEMM on the tensor-core kernel): three fp16 passes (4) and fp16 + two e4m3 correction passes (6)."""
     from segment_anything.predictor import SamPredictor
     cfg = sam_ref.VIT_B
     sd = _sam_sd(cfg, 7202)

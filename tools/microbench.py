@@ -41,7 +41,7 @@ for (M, N, K) in [(64, 2048, 512), (64, 512, 2048), (64, 512, 520), (8, 1040, 51
     us = timeit(f)
     out[f"linear_f32 M{M} N{N} K{K}"] = {"us": round(us, 1), "tflops": round(2 * M * N * K / us / 1e6, 2)}
 
-# ---- tcgen05 GEMM shapes (ViT-H, batch 10), precision 1 and 3
+# ---- tensor-core GEMM shapes (ViT-H, batch 10), precision 1 and 3
 for (M, N, K) in [(49000, 3840, 1280), (49000, 1280, 1280), (40960, 5120, 1280), (40960, 1280, 5120), (40960, 256, 1280), (40960, 1280, 768)]:
     for p in (1, 3):
         asp, bsp = (2 if p >= 3 else 1), (2 if p >= 2 else 1)
