@@ -111,10 +111,32 @@ int sampt_split_f8c(sampt_ctx* ctx, const float* x, int M, int K, void* out, voi
 
 /* softmax(Qx Kx^T) V on tensor cores with pre-extended operands (rel-pos folded into the contraction, see csrc/attn_tc.cu):
  * Qx [BH,Lq,DK], Kx [BH,Lk,DK], Vt [BH,HD,Lkp] fp16; out fp16 [(BH/nheads)*Lq, ld_out] with head h at columns h*HD.
+ * Vt's keys in [Lk, Lkp) are row padding and are never read (they need not be zero or even finite).
  * NT (a key-tile size) is accepted and ignored: the kernel walks the keys in tiles of 64.
  * Replaces Attention.forward + add_decomposed_rel_pos of upstream image_encoder.py. */
 int sampt_attention_f16(sampt_ctx* ctx, const void* Qx, const void* Kx, const void* Vt, int BH, int Lq, int Lk, int Lkp, int DK,
                         int HD, int NT, int nheads, void* out, int ld_out, int split_off, void* stream);
+
+/* ---- unit-test entries, not used by the Python package -------------------------------------------------------------- */
+/* The ViT's tensor-core GEMM (csrc/gemm_tc.cu, csrc/tc_api.cuh) with every option the pipelines use:
+ * C = epilogue(sum over segments i < nseg of A[:, a_off[i] : +K] . B[:, b_off[i] : +K]^T)   (offsets in fp16 units; f8[i] != 0:
+ * the segment holds K e4m3 bytes).  a_off_host / b_off_host / f8_host are HOST int[nseg].  Epilogue, in this order: times
+ * *acc_scale (device float, or NULL), + bias, act (0 none, 1 GELU erf, 3 GELU tanh; anything else is an error), then either
+ * out32 [rows, ldc] (+ resid, read at row % resid_mod when resid_mod > 0; resid may alias out32) or out16 [M, ldc] (bf16 when
+ * is_bf16; split_off > 0: lo = fp16(v - hi) at column split_off, or with out_f8 the e4m3 bytes of (v - hi) 2^12 at byte
+ * 2 split_off + n and of v 2^-3 at byte 3 split_off + n).  rowmap (device int[M] or NULL): destination row of each output
+ * row, -1 = dropped.  skip (device int or NULL): non-zero -> nothing is written. */
+int sampt_test_gemm_tc(sampt_ctx* ctx, const void* A, int lda, const void* B, int ldb, int M, int N, int K, int nseg,
+                       const int* a_off_host, const int* b_off_host, const int* f8_host, const float* bias, int act, int is_bf16,
+                       void* out16, float* out32, const float* resid, int resid_mod, const int* rowmap, const int* skip,
+                       const float* acc_scale, int ldc, int split_off, int out_f8, void* stream);
+/* One ViT attention block between its qkv GEMM and proj (csrc/vit_pipeline.cu): operand preparation (rel-pos folding) then
+ * the attention kernel, scale 1/sqrt(HD), HD = D / nheads.  qkv fp16 [nwb*S*S, 3D] (row = wb*S*S + t, columns q | k | v with
+ * head h at h*HD), rel_pos_h / rel_pos_w fp32 [2S-1, HD].  Caller-owned operands: Qx, Kx fp16 [nwb*nheads, S*S, DK],
+ * Vt fp16 [nwb*nheads, HD, Lkp].  out, ld_out, split_off, out_f8 as in the attention kernel (the A operand of proj). */
+int sampt_test_vit_attention(sampt_ctx* ctx, const void* qkv, const float* rel_pos_h, const float* rel_pos_w, int nwb, int nheads,
+                             int S, int D, int DK, int Lkp, void* Qx, void* Kx, void* Vt, void* out, int ld_out, int split_off,
+                             int out_f8, void* stream);
 
 /* ---- SAM image encoder ------------------------------------------------------------------------------------------ */
 /* ResizeLongestSide.apply_image (PIL bilinear, bit-exact): planar uint8 (B,3,H,W) -> (B,3,Ho,Wo); coefficient tables

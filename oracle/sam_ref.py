@@ -141,22 +141,29 @@ def get_rel_pos(q_size, k_size, rel_pos):
     return rp[rel.long()]
 
 
-def vit_attention(sd: SD, p: str, x, num_heads: int):
-    B, H, W, D = x.shape
-    hd = D // num_heads
+def vit_attention_core(qkv, rel_pos_h, rel_pos_w, H: int, W: int, num_heads: int):
+    """Attention between the qkv and proj linears: qkv (B, H*W, 3D) -> per-head outputs (B, H*W, D), head h at columns
+    h*hd.  Computes in the dtype of its inputs (float64 for kernel tests)."""
+    B, L, D3 = qkv.shape
+    hd = D3 // 3 // num_heads
     scale = hd ** -0.5
-    qkv = F.linear(x, sd[p + "qkv.weight"], sd[p + "qkv.bias"])
-    qkv = qkv.reshape(B, H * W, 3, num_heads, -1).permute(2, 0, 3, 1, 4)
-    q, k, v = qkv.reshape(3, B * num_heads, H * W, -1).unbind(0)
+    qkv = qkv.reshape(B, L, 3, num_heads, -1).permute(2, 0, 3, 1, 4)
+    q, k, v = qkv.reshape(3, B * num_heads, L, -1).unbind(0)
     attn = (q * scale) @ k.transpose(-2, -1)
-    Rh = get_rel_pos(H, H, sd[p + "rel_pos_h"])
-    Rw = get_rel_pos(W, W, sd[p + "rel_pos_w"])
+    Rh = get_rel_pos(H, H, rel_pos_h)
+    Rw = get_rel_pos(W, W, rel_pos_w)
     r_q = q.reshape(B * num_heads, H, W, hd)
     rel_h = torch.einsum("bhwc,hkc->bhwk", r_q, Rh)
     rel_w = torch.einsum("bhwc,wkc->bhwk", r_q, Rw)
     attn = (attn.view(-1, H, W, H, W) + rel_h[:, :, :, :, None] + rel_w[:, :, :, None, :]).view(-1, H * W, H * W)
     attn = attn.softmax(dim=-1)
-    x = (attn @ v).view(B, num_heads, H, W, -1).permute(0, 2, 3, 1, 4).reshape(B, H, W, -1)
+    return (attn @ v).view(B, num_heads, L, -1).permute(0, 2, 1, 3).reshape(B, L, -1)
+
+
+def vit_attention(sd: SD, p: str, x, num_heads: int):
+    B, H, W, D = x.shape
+    qkv = F.linear(x, sd[p + "qkv.weight"], sd[p + "qkv.bias"]).reshape(B, H * W, -1)
+    x = vit_attention_core(qkv, sd[p + "rel_pos_h"], sd[p + "rel_pos_w"], H, W, num_heads).reshape(B, H, W, -1)
     return F.linear(x, sd[p + "proj.weight"], sd[p + "proj.bias"])
 
 

@@ -3,6 +3,7 @@
 // Same outputs (see attn_tc.cu / attn_ws.cu):  Q' = [q*scale | rel_h(q, 0..S-1) | rel_w(q, 0..S-1) | 0]   [BH, L, DK]
 //                                               K' = [k       | onehot(ky)       | onehot(kx)       | 0]   [BH, L, DK]
 //                                               V^T                                                        [BH, HD, Lkp]
+// (keys of V^T in [L, Lkp) are row padding that attn_tc never reads; they are left as they are)
 // with rel_h(q, j) = q . Rh[qy - j + S-1], rel_w(q, j) = q . Rw[qx - j + S-1] (upstream add_decomposed_rel_pos, unscaled q).
 //
 // Round 1 computed the 2S dot products per query on the CUDA cores (440 k FMA per 14x14 window-head, fed from shared memory at
@@ -149,14 +150,6 @@ attn_prep2_kernel(const __half* __restrict__ qkv, int ldq, const __half* __restr
           hv[jj] = (t < nt) ? sv[(size_t)t * QP + d] : __float2half_rn(0.f);
         }
         if (t0 + g * 8 < Lkp) *reinterpret_cast<uint4*>(Vt + (bh * HD + d) * Lkp + t0 + g * 8) = *reinterpret_cast<uint4*>(hv);
-      }
-    }
-    if (t0 + TC >= L) {   // tile padding of V^T (keys in [L, Lkp)) beyond the last written group: zeros, 16 B at a time
-      const int first = ((L - t0 + 7) / 8) * 8 + t0;
-      const int npad8 = max(0, Lkp - first) / 8;
-      for (int i = tid; i < HD * npad8; i += 256) {
-        const int d = i / npad8, t = first + (i % npad8) * 8;
-        *reinterpret_cast<uint4*>(Vt + (bh * HD + d) * Lkp + t) = make_uint4(0u, 0u, 0u, 0u);
       }
     }
   }
@@ -319,14 +312,6 @@ attn_prep2_persistent_kernel(const __half* __restrict__ qkv, int ldq, const __ha
           hv[jj] = (t < nt) ? sv[(size_t)t * QP + d] : __float2half_rn(0.f);
         }
         if (g < ngrp && t0 + g * 8 < Lkp) *reinterpret_cast<uint4*>(Vt + (bh * HD + d) * Lkp + t0 + g * 8) = *reinterpret_cast<uint4*>(hv);
-      }
-      if (t0 + TC >= L) {   // key padding [L, Lkp) of the last chunk
-        const int first = ((L - t0 + 7) / 8) * 8 + t0;
-        const int npad8 = max(0, Lkp - first) / 8;
-        for (int i = tid; i < HD * npad8; i += 256) {
-          const int d = i / npad8, t = first + (i % npad8) * 8;
-          *reinterpret_cast<uint4*>(Vt + (bh * HD + d) * Lkp + t) = make_uint4(0u, 0u, 0u, 0u);
-        }
       }
     }
     // ---- T[TC x NRP] = q . Rcat^T (mma.sync m16n8k16, fp32 accumulate, Rcat = hi + lo); 4 m-tiles x 2 column halves over 8 warps

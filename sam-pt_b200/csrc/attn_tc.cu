@@ -229,7 +229,9 @@ int attn_tc(Ctx* c, cudaStream_t st, const __half* Qx, const __half* Kx, const _
   CUtensorMap tmQ, tmK, tmV;
   SAMPT_TRY(make_tmap_3d_f16(&tmQ, Qx, DK, Lq, BH, (uint64_t)DK * 2, (uint64_t)Lq * DK * 2, 64, 128, 1));
   SAMPT_TRY(make_tmap_3d_f16(&tmK, Kx, DK, Lk, BH, (uint64_t)DK * 2, (uint64_t)Lk * DK * 2, 64, A_KT, 1));
-  SAMPT_TRY(make_tmap_3d_f16(&tmV, Vt, Lkp, HD, BH, (uint64_t)Lkp * 2, (uint64_t)HD * Lkp * 2, 64, HD, 1));
+  // V^T rows have the pitch Lkp but only Lk valid keys: TMA zero-fills the tail of the last tile, so whatever the padding
+  // [Lk, Lkp) holds never meets a P = 0 (0 * NaN would poison the row)
+  SAMPT_TRY(make_tmap_3d_f16(&tmV, Vt, Lk, HD, BH, (uint64_t)Lkp * 2, (uint64_t)HD * Lkp * 2, 64, HD, 1));
   AttnParams p;
   p.Lq = Lq; p.Lk = Lk; p.DKB = DK / 64; p.HD = HD; p.nheads = nheads; p.stages = 2;
   p.out = out; p.ld_out = ld_out; p.split_off = split_off; p.out_f8 = out_f8;
@@ -255,4 +257,18 @@ extern "C" int sampt_attention_f16(sampt_ctx* ctx, const void* Qx, const void* K
   return attn_tc(reinterpret_cast<Ctx*>(ctx), reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const __half*>(Qx),
                  reinterpret_cast<const __half*>(Kx), reinterpret_cast<const __half*>(Vt), BH, Lq, Lk, Lkp, DK, HD, nheads,
                  reinterpret_cast<__half*>(out), ld_out, split_off);
+}
+
+// Unit-test entry: what one ViT block runs between its qkv GEMM and proj (vit_pipeline.cu): attn_prep + attn_tc, scale 1/sqrt(HD).
+extern "C" int sampt_test_vit_attention(sampt_ctx* ctx, const void* qkv, const float* rel_pos_h, const float* rel_pos_w, int nwb,
+                                        int nheads, int S, int D, int DK, int Lkp, void* Qx, void* Kx, void* Vt, void* out, int ld_out,
+                                        int split_off, int out_f8, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(nheads > 0 && D % nheads == 0, "sampt_test_vit_attention: D (%d) must be a multiple of nheads (%d)", D, nheads);
+  const int HD = D / nheads, L = S * S;
+  __half *q = reinterpret_cast<__half*>(Qx), *k = reinterpret_cast<__half*>(Kx), *v = reinterpret_cast<__half*>(Vt);
+  SAMPT_TRY(attn_prep(c, st, reinterpret_cast<const __half*>(qkv), 3 * D, rel_pos_h, rel_pos_w, q, k, v, nwb, nheads, S, Lkp, DK, D, HD,
+                      1.0f / sqrtf((float)HD)));
+  return attn_tc(c, st, q, k, v, nwb * nheads, L, L, Lkp, DK, HD, nheads, reinterpret_cast<__half*>(out), ld_out, split_off, out_f8);
 }

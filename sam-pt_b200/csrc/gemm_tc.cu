@@ -174,6 +174,7 @@ int gemm_tc(Ctx* c, cudaStream_t st, const void* A, int lda, const void* B, int 
   SAMPT_CHECK(seg.nseg >= 1 && seg.nseg <= 3, "gemm_tc: nseg out of range");
   SAMPT_CHECK((ep.out16 != nullptr) != (ep.out32 != nullptr), "gemm_tc: exactly one of out16/out32 must be set");
   SAMPT_CHECK(ep.ldc % 8 == 0, "gemm_tc: ldc must be a multiple of 8");
+  SAMPT_CHECK(ep.act == 0 || ep.act == 1 || ep.act == 3, "gemm_tc: act %d is not 0 (none), 1 (GELU erf) or 3 (GELU tanh)", ep.act);
   const bool f8 = (seg.f8[0] | seg.f8[1] | seg.f8[2]) != 0;
   SAMPT_CHECK(!f8 || K % (2 * G_BK) == 0, "gemm_tc: e4m3 segments need K %% 128 == 0 (K = %d)", K);
   SAMPT_CHECK(!f8 || !ep.is_bf16, "gemm_tc: e4m3 segments go with fp16 operands");
@@ -248,6 +249,32 @@ extern "C" int sampt_gemm_f8c(sampt_ctx* ctx, const void* A, const void* B, int 
   ep.out_f8 = out_f8;
   ep.acc_scale = acc_scale_dev;
   return gemm_tc(c, reinterpret_cast<cudaStream_t>(stream), A, 2 * K, B, 2 * K, M, N, K, make_seg_f8(K), ep);
+}
+
+// Unit-test entry: gemm_tc with every GemmSeg / GemmEpi field supplied by the caller (include/sampt_b200.h).
+extern "C" int sampt_test_gemm_tc(sampt_ctx* ctx, const void* A, int lda, const void* B, int ldb, int M, int N, int K, int nseg,
+                                  const int* a_off_host, const int* b_off_host, const int* f8_host, const float* bias, int act,
+                                  int is_bf16, void* out16, float* out32, const float* resid, int resid_mod, const int* rowmap,
+                                  const int* skip, const float* acc_scale, int ldc, int split_off, int out_f8, void* stream) {
+  SAMPT_CHECK(nseg >= 1 && nseg <= 3, "sampt_test_gemm_tc: nseg %d out of range", nseg);
+  GemmSeg seg{};
+  seg.nseg = nseg;
+  for (int i = 0; i < nseg; ++i) { seg.a_off[i] = a_off_host[i]; seg.b_off[i] = b_off_host[i]; seg.f8[i] = f8_host[i]; }
+  GemmEpi ep{};
+  ep.out16 = reinterpret_cast<__half*>(out16);
+  ep.out32 = out32;
+  ep.resid = resid;
+  ep.bias = bias;
+  ep.rowmap = rowmap;
+  ep.ldc = ldc;
+  ep.act = act;
+  ep.split_off = split_off;
+  ep.is_bf16 = is_bf16;
+  ep.resid_mod = resid_mod;
+  ep.skip = skip;
+  ep.acc_scale = acc_scale;
+  ep.out_f8 = out_f8;
+  return gemm_tc(reinterpret_cast<Ctx*>(ctx), reinterpret_cast<cudaStream_t>(stream), A, lda, B, ldb, M, N, K, seg, ep);
 }
 
 // x [M, K] fp32 -> the A operand of sampt_gemm_f8c: [fp16(x) | e4m3((x - fp16(x)) * 2^12) | e4m3(x * 2^-3)], 2K fp16 units per row

@@ -207,6 +207,7 @@ int ln_rows(Ctx* c, cudaStream_t st, const float* x, int ldx, const int* src, co
 // ---------------------------------------------------------------------------------------------------------------------
 // Attention operand preparation (see attn_tc.cu): from qkv [Mrows, 3*D] fp16 (row = wb*L + t) build
 //   Qx [BH, L, DK], Kx [BH, L, DK], Vt [BH, HD, Lkp]     BH = nwb * nheads, L = S*S tokens, token t = ty*S + tx
+// (V^T keys in [L, Lkp) are row padding that attn_tc never reads)
 // One CTA per (chunk of TC tokens sharing rows of the grid, head, wb).  Register tiled 4x4 (t, j) dot products.
 // ---------------------------------------------------------------------------------------------------------------------
 template <int HD>
@@ -283,14 +284,6 @@ attn_prep_kernel(const __half* __restrict__ qkv, int ldq, const float* __restric
         hv[j] = (t < nt) ? sv[(size_t)t * QP + d] : __float2half_rn(0.f);
       }
       if (t0 + g * 8 < Lkp) *reinterpret_cast<uint4*>(Vt + (bh * HD + d) * Lkp + t0 + g * 8) = *reinterpret_cast<uint4*>(hv);
-    }
-    // the tile padding of V^T (keys in [L, Lkp)) beyond the last written group: zeros, written by the last chunk
-    if (t0 + TC >= L) {
-      const int first = ((L - t0 + 7) / 8) * 8 + t0;  // first key not covered by the groups above
-      for (int i = tid; i < HD * max(0, Lkp - first); i += 256) {
-        const int d = i / (Lkp - first), t = first + i % (Lkp - first);
-        Vt[(bh * HD + d) * Lkp + t] = __float2half_rn(0.f);
-      }
     }
   }
   // ---- phase 2: rel_h(q, j) = q . Rh[ty - j + S-1] ; rel_w(q, j) = q . Rw[tx - j + S-1]
