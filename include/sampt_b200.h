@@ -118,6 +118,8 @@ int sampt_attention_f16(sampt_ctx* ctx, const void* Qx, const void* Kx, const vo
                         int HD, int NT, int nheads, void* out, int ld_out, int split_off, void* stream);
 
 /* ---- unit-test entries, not used by the Python package -------------------------------------------------------------- */
+/* Six entries: the ViT's tensor-core GEMM and attention block (below), then four stages of the SAM prompt encoder / mask
+ * decoder (attention cores, prompt encoder, upscaling tail, postprocess + refinement control). */
 /* The ViT's tensor-core GEMM (csrc/gemm_tc.cu, csrc/tc_api.cuh) with every option the pipelines use:
  * C = epilogue(sum over segments i < nseg of A[:, a_off[i] : +K] . B[:, b_off[i] : +K]^T)   (offsets in fp16 units; f8[i] != 0:
  * the segment holds K e4m3 bytes).  a_off_host / b_off_host / f8_host are HOST int[nseg].  Epilogue, in this order: times
@@ -137,6 +139,31 @@ int sampt_test_gemm_tc(sampt_ctx* ctx, const void* A, int lda, const void* B, in
 int sampt_test_vit_attention(sampt_ctx* ctx, const void* qkv, const float* rel_pos_h, const float* rel_pos_w, int nwb, int nheads,
                              int S, int D, int DK, int Lkp, void* Qx, void* Kx, void* Vt, void* out, int ld_out, int split_off,
                              int out_f8, void* stream);
+/* One SAM decoder attention core (csrc/decoder.cu), 8 heads, on caller-owned fp32 buffers, scale 1/sqrt(head dim):
+ *   kind 0: token self-attention, block per (token, head) (the decode chain's kernel for T <= 16), head dim 32: q, k, v,
+ *           out [T, 256], Nk == T;
+ *   kind 1: token self-attention, warp per query (the chain's kernel for T > 16), same layout; T up to the shared-memory limit;
+ *   kind 2: tokens -> image, head dim 16: q, out [T, 128], k, v [Nk, 128]; keys split in slices of 256, then combined
+ *           (partials in the ctx workspace);
+ *   kind 3: image -> tokens, head dim 16: q, out [Nk, 128] (Nk image tokens), k, v [T, 128] (T prompt tokens). */
+int sampt_test_sam_attention(sampt_ctx* ctx, int kind, const float* q, const float* k, const float* v, float* out, int T, int Nk,
+                             void* stream);
+/* The prompt encoder as the decode chain runs it, with the registered decoder weights: coords (K,2) in the 1024 frame, labels (K)
+ * int32, box (4) or NULL, mask_in (256*256) or NULL -> tokens_out [T,256] = output tokens ++ point tokens ++ (pad point | two box
+ * corners), src_out [G*G,256] = feat_tok + dense embedding (mask_downscaling(mask_in), or no_mask_embed). */
+int sampt_test_sam_prompt(sampt_ctx* ctx, const float* feat_tok, int G, const float* coords, const int* labels, int K, const float* box,
+                          const float* mask_in, float* tokens_out, float* src_out, void* stream);
+/* The mask decoder's upscaling tail after its first ConvT: u1 [G*G, 4*64] (row = token, column = (dy*2+dx)*64 + c) -> LayerNorm2d,
+ * GELU, ConvT(64->32, k2 s2), GELU, dot with hyper [n_masks, 32] (1 <= n_masks <= 4) -> low_res [n_masks, 4G, 4G]; u_out
+ * [(4G)^2, 32] receives the upscaled embedding when not NULL. */
+int sampt_test_sam_upscale(sampt_ctx* ctx, const float* u1, const float* hyper, int n_masks, int G, float* low_res, float* u_out,
+                           void* stream);
+/* Sam.postprocess_masks and one step of the refinement control: low_res [n_masks, 4G, 4G] -> out [n_masks, H, W] (bilinear to
+ * 16G, crop to in_h x in_w, bilinear to H x W); bbox5 (device int[5]) = xmin, ymin, xmax, ymax, count of out[0] > 0 as
+ * accumulated; then the chain's break test: skip (device int) = 1 when count < 2, else box4 (device float[4]) = the box and
+ * n_done (device int) = 1. */
+int sampt_test_sam_postprocess(sampt_ctx* ctx, const float* low_res, int n_masks, int G, int in_h, int in_w, int H, int W, float* out,
+                               int* bbox5, float* box4, int* skip, int* n_done, void* stream);
 
 /* ---- SAM image encoder ------------------------------------------------------------------------------------------ */
 /* ResizeLongestSide.apply_image (PIL bilinear, bit-exact): planar uint8 (B,3,H,W) -> (B,3,Ho,Wo); coefficient tables

@@ -25,7 +25,8 @@ independent implementation that exists in this image
 (``transformers.models.sam``) by ``tests/test_oracle_sam_vs_hf.py`` via a key
 remap — see that test.
 
-Everything is float32 torch on CPU, written for clarity not speed.
+Everything is torch on CPU, written for clarity not speed: float32 as upstream, and the prompt encoder, mask decoder and
+``postprocess_masks`` follow the dtype of the state dict and inputs (float64 for the decoder's kernel tests).
 """
 from __future__ import annotations
 
@@ -234,7 +235,7 @@ def _pe_encoding(sd: SD, coords, prefix="prompt_encoder."):
 
 def get_dense_pe(sd: SD, emb_hw=(64, 64), prefix="prompt_encoder."):
     h, w = emb_hw
-    grid = torch.ones((h, w), dtype=torch.float32)
+    grid = torch.ones((h, w), dtype=sd[prefix + "pe_layer.positional_encoding_gaussian_matrix"].dtype)
     y_embed = (grid.cumsum(dim=0) - 0.5) / h
     x_embed = (grid.cumsum(dim=1) - 0.5) / w
     pe = _pe_encoding(sd, torch.stack([x_embed, y_embed], dim=-1), prefix)
@@ -245,13 +246,14 @@ def _pe_with_coords(sd, coords, image_size, prefix):
     coords = coords.clone()
     coords[:, :, 0] = coords[:, :, 0] / image_size[1]
     coords[:, :, 1] = coords[:, :, 1] / image_size[0]
-    return _pe_encoding(sd, coords.float(), prefix)
+    return _pe_encoding(sd, coords.to(sd[prefix + "pe_layer.positional_encoding_gaussian_matrix"].dtype), prefix)
 
 
 def prompt_encode(sd: SD, points, boxes, masks, img_size=1024, emb_hw=(64, 64), prefix="prompt_encoder."):
     """points = (coords (B,K,2) float in the 1024 frame, labels (B,K) int) or None; boxes (B,4)/(B,1,4) or None;
-    masks (B,1,256,256) or None.  Returns sparse (B,K',256), dense (B,256,64,64)."""
+    masks (B,1,256,256) or None.  Returns sparse (B,K',256), dense (B,256,64,64), in the dtype of the state dict."""
     p = prefix
+    dt = sd[p + "pe_layer.positional_encoding_gaussian_matrix"].dtype
     bs = 1
     if points is not None:
         bs = points[0].shape[0]
@@ -259,12 +261,12 @@ def prompt_encode(sd: SD, points, boxes, masks, img_size=1024, emb_hw=(64, 64), 
         bs = boxes.shape[0]
     elif masks is not None:
         bs = masks.shape[0]
-    sparse = torch.empty((bs, 0, 256))
+    sparse = torch.empty((bs, 0, 256), dtype=dt)
     if points is not None:
         coords, labels = points
         coords = coords + 0.5
         if boxes is None:
-            coords = torch.cat([coords, torch.zeros((bs, 1, 2))], dim=1)
+            coords = torch.cat([coords, torch.zeros((bs, 1, 2), dtype=coords.dtype)], dim=1)
             labels = torch.cat([labels, -torch.ones((bs, 1), dtype=labels.dtype)], dim=1)
         pe = _pe_with_coords(sd, coords, (img_size, img_size), p)
         pe[labels == -1] = 0.0

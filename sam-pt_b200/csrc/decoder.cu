@@ -43,10 +43,14 @@ prompt_tokens_kernel(PromptArgs a, float* __restrict__ tokens, const int* skip) 
   if (t < a.n_out_tok) { out[ch] = a.out_tokens[(size_t)t * 256 + ch]; return; }
   const int i = t - a.n_out_tok;
   float x, y;
-  int label;  // -1 pad, 0 neg, 1 pos, 2/3 box corners
-  if (i < a.K) { x = a.coords[2 * i]; y = a.coords[2 * i + 1]; label = a.labels[i]; }
-  else if (!a.use_box) { x = 0.f; y = 0.f; label = -1; }
-  else { int cidx = i - a.K; x = a.box[2 * cidx]; y = a.box[2 * cidx + 1]; label = 2 + cidx; }
+  int label;                       // -1: not a point (user label -1 or the pad point)
+  const float* emb = nullptr;      // learned embedding added to the PE: point_embeddings[0|1] for user labels 0 / 1, [2|3] for
+                                   // the box corners; any other user label gets the PE alone (upstream PromptEncoder._embed_points)
+  if (i < a.K) {
+    x = a.coords[2 * i]; y = a.coords[2 * i + 1]; label = a.labels[i];
+    if (label == 0 || label == 1) emb = a.pt_emb[label];
+  } else if (!a.use_box) { x = 0.f; y = 0.f; label = -1; }
+  else { int cidx = i - a.K; x = a.box[2 * cidx]; y = a.box[2 * cidx + 1]; label = 2 + cidx; emb = a.pt_emb[2 + cidx]; }
   // +0.5 (pixel centre), normalise to [0,1], 2c-1, @ G, * 2pi, [sin | cos]
   x = (x + 0.5f) / a.img_size; y = (y + 0.5f) / a.img_size;
   float cx = 2.f * x - 1.f, cy = 2.f * y - 1.f;
@@ -55,7 +59,7 @@ prompt_tokens_kernel(PromptArgs a, float* __restrict__ tokens, const int* skip) 
   v = 2.0f * 3.14159265358979323846f * v;
   float pe = (ch < 128) ? sinf(v) : cosf(v);
   if (label == -1) pe = a.not_a_point[ch];
-  else pe += a.pt_emb[label][ch];
+  else if (emb != nullptr) pe += emb[ch];
   out[ch] = pe;
 }
 
@@ -891,6 +895,40 @@ static int tcg(Ctx* c, cudaStream_t st, const __half* X16, const __half* W16, co
   return gemm_tc(c, st, X16, 2 * K, W16, 2 * K, M, N, K, seg, ep);
 }
 
+// The attention cores of the decoder, 8 heads.  Each launcher is shared by the decode chain and the unit-test entries.
+// Token self-attention, head dim 32 (q/k/v/out [T, 256]): kind 0 = attn_q_small_kernel (block per token and head), the chain's
+// choice for T <= 16; kind 1 = attn_tok_self_kernel (warp per query, the head's K/V in dynamic shared memory).
+static int launch_tok_self(Ctx* c, cudaStream_t st, int kind, const float* q, const float* k, const float* v, float* out, int T,
+                           const int* skip) {
+  if (kind == 1) {
+    const size_t smem = ((size_t)2 * T * 33 + (size_t)8 * T + 8 * 32) * sizeof(float);
+    SAMPT_CHECK(smem <= 200 * 1024, "too many prompt tokens (%d) for the token self-attention", T);
+    SAMPT_TRY(ensure_func_smem(c, "attn_tok_self_kernel<32>", attn_tok_self_kernel<32>, 200 * 1024));
+    attn_tok_self_kernel<32><<<dim3(cdiv(T, 32), 8), 256, smem, st>>>(q, k, v, out, T, 8, skip);
+  } else {
+    attn_q_small_kernel<32><<<dim3(T, 8), 256, 0, st>>>(q, k, v, out, T, 8, skip);
+  }
+  LAUNCH_OK();
+  return 0;
+}
+// Tokens -> image, head dim 16: q [T, 128] over k/v [Nk, 128], split over the keys in slices of 256 (part: T*8*nsplit*18 floats).
+static int launch_t2i(Ctx* c, cudaStream_t st, const float* q, const float* k, const float* v, float* part, float* out, int T, int Nk,
+                      const int* skip) {
+  constexpr int KPS = 256;
+  const int nsplit = (Nk + KPS - 1) / KPS;
+  attn_t2i_partial_kernel<16, KPS><<<dim3(nsplit, 8), 256, 0, st>>>(q, k, v, part, T, Nk, 8, skip);
+  LAUNCH_OK();
+  attn_t2i_combine_kernel<16><<<cdiv(T * 128, 128), 128, 0, st>>>(part, out, T, 8, nsplit, skip);
+  LAUNCH_OK();
+  return 0;
+}
+// Image -> tokens, head dim 16: q [N, 128] over k/v [T, 128].
+static int launch_i2t(Ctx* c, cudaStream_t st, const float* q, const float* k, const float* v, float* out, int N, int T, const int* skip) {
+  attn_kv_small_kernel<16><<<cdiv((long long)cdiv(N, 32) * 8, 8), 256, 0, st>>>(q, k, v, out, N, T, 8, skip);
+  LAUNCH_OK();
+  return 0;
+}
+
 // tokens -> image attention: queries attend over the 4096 image tokens.  q_in already includes the query PE.
 static int attn_tok_to_img(Ctx* c, cudaStream_t st, const AttnW& a, const float* q_in, const float* keys, const float* pek,
                            DecBufs& b, float* out /*[T,256]*/, const float* resid, int GG, const int* skip) {
@@ -903,14 +941,7 @@ static int attn_tok_to_img(Ctx* c, cudaStream_t st, const AttnW& a, const float*
     SAMPT_TRY(sg(c, st, keys, 256, a.kw, a.kb, pek, 128, b.ik, 128, GG, 128, 256, 0, skip));   // (keys + key_pe) Wk^T
     SAMPT_TRY(sg(c, st, keys, 256, a.vw, a.vb, nullptr, 0, b.iv, 128, GG, 128, 256, 0, skip));
   }
-  {
-    constexpr int KPS = 256;
-    const int nsplit = (GG + KPS - 1) / KPS;
-    attn_t2i_partial_kernel<16, KPS><<<dim3(nsplit, 8), 256, 0, st>>>(b.tq, b.ik, b.iv, b.part, T, GG, 8, skip);
-    LAUNCH_OK();
-    attn_t2i_combine_kernel<16><<<cdiv(T * 128, 128), 128, 0, st>>>(b.part, b.ta, T, 8, nsplit, skip);
-    LAUNCH_OK();
-  }
+  SAMPT_TRY(launch_t2i(c, st, b.tq, b.ik, b.iv, b.part, b.ta, T, GG, skip));
   SAMPT_TRY(sg(c, st, b.ta, 128, a.ow, a.ob, resid, 256, out, 256, T, 256, 128, 0, skip));
   return 0;
 }
@@ -928,15 +959,7 @@ static int two_way_layer(Ctx* c, cudaStream_t st, const LayerW& L, int idx, DecB
     SAMPT_TRY(sg(c, st, b.qpe, 256, L.self_attn.kw, L.self_attn.kb, nullptr, 0, b.tk, 256, T, 256, 256, 0, skip));
   }
   SAMPT_TRY(sg(c, st, b.queries, 256, L.self_attn.vw, L.self_attn.vb, nullptr, 0, b.tv, 256, T, 256, 256, 0, skip));
-  if (T > 16) {
-    const size_t smem = ((size_t)2 * T * 33 + (size_t)8 * T + 8 * 32) * sizeof(float);
-    SAMPT_CHECK(smem <= 200 * 1024, "too many prompt tokens (%d) for the token self-attention", T);
-    SAMPT_TRY(ensure_func_smem(c, "attn_tok_self_kernel<32>", attn_tok_self_kernel<32>, 200 * 1024));
-    attn_tok_self_kernel<32><<<dim3(cdiv(T, 32), 8), 256, smem, st>>>(b.tq, b.tk, b.tv, b.ta, T, 8, skip);
-  } else {
-    attn_q_small_kernel<32><<<dim3(T, 8), 256, 0, st>>>(b.tq, b.tk, b.tv, b.ta, T, 8, skip);
-  }
-  LAUNCH_OK();
+  SAMPT_TRY(launch_tok_self(c, st, T > 16 ? 1 : 0, b.tq, b.tk, b.tv, b.ta, T, skip));
   // layer 0 replaces the queries, later layers add (upstream skip_first_layer_pe)
   SAMPT_TRY(sg(c, st, b.ta, 256, L.self_attn.ow, L.self_attn.ob, idx == 0 ? nullptr : b.queries, 256, b.tmp, 256, T, 256, 256, 0, skip));
   ln256_kernel<<<cdiv(T, 8), 256, 0, st>>>(b.tmp, nullptr, L.n1w, L.n1b, b.queries, T, 1e-5f, skip);
@@ -959,8 +982,7 @@ static int two_way_layer(Ctx* c, cudaStream_t st, const LayerW& L, int idx, DecB
   else SAMPT_TRY(sg(c, st, b.keys, 256, L.i2t.qw, L.i2t.qb, L.peq_i2t, 128, b.iq, 128, GG, 128, 256, 0, skip));  // (keys+pe) Wq^T
   SAMPT_TRY(sg(c, st, b.qpe, 256, L.i2t.kw, L.i2t.kb, nullptr, 0, b.tk, 128, T, 128, 256, 0, skip));
   SAMPT_TRY(sg(c, st, b.queries, 256, L.i2t.vw, L.i2t.vb, nullptr, 0, b.tv, 128, T, 128, 256, 0, skip));
-  attn_kv_small_kernel<16><<<cdiv((long long)cdiv(GG, 32) * 8, 8), 256, 0, st>>>(b.iq, b.tk, b.tv, b.ia, GG, T, 8, skip);
-  LAUNCH_OK();
+  SAMPT_TRY(launch_i2t(c, st, b.iq, b.tk, b.tv, b.ia, GG, T, skip));
   if (L.i2t.ow16 != nullptr) {
     SAMPT_TRY(split_rows(c, st, b.ia, b.ia16, GG, 128, skip));
     SAMPT_TRY(tcg(c, st, b.ia16, L.i2t.ow16, L.i2t.ob, b.keys, b.src, 256, GG, 256, 128, skip));          // keys + attn_out
@@ -988,16 +1010,38 @@ struct DecodeCall {
   const float* hq_feat;      // [256*256][32] HQ features of this frame, or null (plain SAM)
 };
 
+// prompt encoder: sparse tokens [T, 256] (output tokens first) and src = image embedding + dense embedding [G*G, 256]
+static int encode_prompt(Ctx* c, cudaStream_t st, const DecW& w, const DecodeCall& d, int G, float* tokens, float* src) {
+  const int T = w.n_out_tok + d.K + (d.use_box ? 2 : 1);
+  PromptArgs pa = w.prompt;
+  pa.coords = d.coords; pa.labels = d.labels; pa.K = d.K; pa.box = d.box; pa.use_box = d.use_box; pa.img_size = (float)(G * 16);
+  prompt_tokens_kernel<<<T, 256, 0, st>>>(pa, tokens, d.skip);
+  LAUNCH_OK();
+  dense_src_kernel<<<cdiv(G * G, 8), 256, 0, st>>>(d.feat_tok, d.mask_in, w.dense, src, G, d.skip);
+  LAUNCH_OK();
+  return 0;
+}
+// LN2d + GELU + ConvT(64->32) + GELU + hyper-network dot on the first ConvT's output u1 [G*G, 4*64] -> low_res [n_masks, 4G, 4G]
+static int launch_upscale(Ctx* c, cudaStream_t st, const DecW& w, const float* u1, const float* hyper, int n_masks, float* low_res,
+                          int G, float* u_out, const int* skip) {
+  upscale_mask_kernel<<<cdiv(16 * G * G, 256), 256, 0, st>>>(u1, w.up_lnw, w.up_lnb, w.up3_w, w.up3_b, hyper, n_masks, low_res, G,
+                                                             u_out, skip);
+  LAUNCH_OK();
+  return 0;
+}
+static int launch_postprocess(Ctx* c, cudaStream_t st, const float* low_res, int n_masks, int G, int in_h, int in_w, int H, int W,
+                              float* out, int* bbox, const int* skip) {
+  postprocess_kernel<<<cdiv((long long)n_masks * H * W, 256), 256, 0, st>>>(low_res, n_masks, 4 * G, 16 * G, in_h, in_w, H, W, out,
+                                                                           bbox, skip);
+  LAUNCH_OK();
+  return 0;
+}
+
 static int decode_once(Ctx* c, cudaStream_t st, DecW& w, DecBufs& b, const DecodeCall& d, int G) {
   const int GG = G * G;
   const int T = w.n_out_tok + d.K + (d.use_box ? 2 : 1);
   b.T = T;
-  PromptArgs pa = w.prompt;
-  pa.coords = d.coords; pa.labels = d.labels; pa.K = d.K; pa.box = d.box; pa.use_box = d.use_box; pa.img_size = (float)(G * 16);
-  prompt_tokens_kernel<<<T, 256, 0, st>>>(pa, b.tokens, d.skip);
-  LAUNCH_OK();
-  dense_src_kernel<<<cdiv(GG, 8), 256, 0, st>>>(d.feat_tok, d.mask_in, w.dense, b.keys, G, d.skip);
-  LAUNCH_OK();
+  SAMPT_TRY(encode_prompt(c, st, w, d, G, b.tokens, b.keys));
   SAMPT_CUDA(cudaMemcpyAsync(b.queries, b.tokens, (size_t)T * 256 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (w.tc) SAMPT_TRY(split_rows(c, st, b.keys, b.keys16, GG, 256, d.skip));
   for (int i = 0; i < 2; ++i) SAMPT_TRY(two_way_layer(c, st, w.layer[i], i, b, GG, d.skip));
@@ -1031,9 +1075,7 @@ static int decode_once(Ctx* c, cudaStream_t st, DecW& w, DecBufs& b, const Decod
   // upscaling: ConvT(256->64) as GEMM [GG,256] x [256(4 sub-pixels x 64), 256]^T, then fused LN+GELU+ConvT+GELU+hyper dot
   if (w.tc) SAMPT_TRY(tcg(c, st, b.keys16, w.up0_w16, w.up0_b4, nullptr, b.u1, 256, GG, 256, 256, d.skip));
   else SAMPT_TRY(sg(c, st, b.keys, 256, w.up0_w, w.up0_b4, nullptr, 0, b.u1, 256, GG, 256, 256, 0, d.skip));
-  upscale_mask_kernel<<<cdiv(16 * GG, 256), 256, 0, st>>>(b.u1, w.up_lnw, w.up_lnb, w.up3_w, w.up3_b, b.hyper, d.n_masks, d.low_res,
-                                                         G, hq ? b.u_sam : nullptr, d.skip);
-  LAUNCH_OK();
+  SAMPT_TRY(launch_upscale(c, st, w, b.u1, b.hyper, d.n_masks, d.low_res, G, hq ? b.u_sam : nullptr, d.skip));
   if (hq) {
     // upscaled_embedding_hq = embedding_maskfeature(upscaled_embedding_sam) + hq_features ; mask += hyper_hq . that
     const int R = 4 * G;
@@ -1044,9 +1086,7 @@ static int decode_once(Ctx* c, cudaStream_t st, DecW& w, DecBufs& b, const Decod
     hq_mask_add_kernel<<<cdiv(R * R, 256), 256, 0, st>>>(b.mf2, d.hq_feat, b.hyper + 4 * 32, d.low_res, R * R, d.skip);
     LAUNCH_OK();
   }
-  postprocess_kernel<<<cdiv((long long)d.n_masks * d.H * d.W, 256), 256, 0, st>>>(d.low_res, d.n_masks, 4 * G, 16 * G, d.in_h, d.in_w,
-                                                                                 d.H, d.W, d.logits, d.bbox, d.skip);
-  LAUNCH_OK();
+  SAMPT_TRY(launch_postprocess(c, st, d.low_res, d.n_masks, G, d.in_h, d.in_w, d.H, d.W, d.logits, d.bbox, d.skip));
   // iou predictions of the selected tokens
   SAMPT_CUDA(cudaMemcpyAsync(d.iou, b.iou4 + d.tok0, d.n_masks * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
@@ -1381,5 +1421,65 @@ extern "C" int sampt_sam_hq_features(sampt_ctx* ctx, const float* feat_tok, cons
 // Select the HQ features used by subsequent sampt_sam_predict / sampt_sam_predict_refine calls (NULL = plain SAM masks).
 extern "C" int sampt_sam_set_hq_features(sampt_ctx* ctx, const float* hq_features) {
   reinterpret_cast<Ctx*>(ctx)->hq_feat = hq_features;
+  return 0;
+}
+
+// ---- unit-test entries: one decoder stage on caller buffers, through the same launchers as the decode chain -------------------
+extern "C" int sampt_test_sam_attention(sampt_ctx* ctx, int kind, const float* q, const float* k, const float* v, float* out, int T,
+                                        int Nk, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(T >= 1 && Nk >= 1, "sampt_test_sam_attention: T (%d) and Nk (%d) must be positive", T, Nk);
+  switch (kind) {
+    case 0:
+    case 1:
+      SAMPT_CHECK(Nk == T, "sampt_test_sam_attention: token self-attention needs Nk == T (got %d, %d)", Nk, T);
+      return launch_tok_self(c, st, kind, q, k, v, out, T, nullptr);
+    case 2: {
+      c->ws_reset();
+      float* part;
+      SAMPT_TRY(ws_get(c, &part, (size_t)T * 8 * ((Nk + 255) / 256) * 18, "attention partials"));
+      return launch_t2i(c, st, q, k, v, part, out, T, Nk, nullptr);
+    }
+    case 3:
+      return launch_i2t(c, st, q, k, v, out, Nk, T, nullptr);
+    default:
+      set_error("sampt_test_sam_attention: unknown kind %d", kind);
+      return -2;
+  }
+}
+
+extern "C" int sampt_test_sam_prompt(sampt_ctx* ctx, const float* feat_tok, int G, const float* coords, const int* labels, int K,
+                                     const float* box, const float* mask_in, float* tokens_out, float* src_out, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  DecW w;
+  SAMPT_TRY(load_dec(c, &w));
+  DecodeCall d{};
+  d.feat_tok = feat_tok; d.coords = coords; d.labels = labels; d.K = K; d.box = box; d.use_box = box ? 1 : 0; d.mask_in = mask_in;
+  return encode_prompt(c, reinterpret_cast<cudaStream_t>(stream), w, d, G, tokens_out, src_out);
+}
+
+extern "C" int sampt_test_sam_upscale(sampt_ctx* ctx, const float* u1, const float* hyper, int n_masks, int G, float* low_res,
+                                      float* u_out, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  SAMPT_CHECK(n_masks >= 1 && n_masks <= 4, "sampt_test_sam_upscale: n_masks %d out of [1, 4]", n_masks);
+  DecW w;
+  SAMPT_TRY(load_dec(c, &w));
+  return launch_upscale(c, reinterpret_cast<cudaStream_t>(stream), w, u1, hyper, n_masks, low_res, G, u_out, nullptr);
+}
+
+extern "C" int sampt_test_sam_postprocess(sampt_ctx* ctx, const float* low_res, int n_masks, int G, int in_h, int in_w, int H, int W,
+                                          float* out, int* bbox5, float* box4, int* skip, int* n_done, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  c->ws_reset();
+  int* acc;   // the chain's accumulator; refine_ctl_kernel resets it, so the caller gets a copy taken before that
+  SAMPT_TRY(ws_get(c, &acc, 8, "bbox"));
+  init_ctl_kernel<<<1, 1, 0, st>>>(acc, skip, n_done);
+  LAUNCH_OK();
+  SAMPT_TRY(launch_postprocess(c, st, low_res, n_masks, G, in_h, in_w, H, W, out, acc, nullptr));
+  SAMPT_CUDA(cudaMemcpyAsync(bbox5, acc, 5 * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  refine_ctl_kernel<<<1, 1, 0, st>>>(acc, box4, skip, n_done);
+  LAUNCH_OK();
   return 0;
 }
