@@ -118,8 +118,8 @@ int sampt_attention_f16(sampt_ctx* ctx, const void* Qx, const void* Kx, const vo
                         int HD, int NT, int nheads, void* out, int ld_out, int split_off, void* stream);
 
 /* ---- unit-test entries, not used by the Python package -------------------------------------------------------------- */
-/* Six entries: the ViT's tensor-core GEMM and attention block (below), then four stages of the SAM prompt encoder / mask
- * decoder (attention cores, prompt encoder, upscaling tail, postprocess + refinement control). */
+/* Eleven entries: the ViT's tensor-core GEMM and attention block (below), four stages of the SAM prompt encoder / mask
+ * decoder (attention cores, prompt encoder, upscaling tail, postprocess + refinement control), then five of the PIPS tracker. */
 /* The ViT's tensor-core GEMM (csrc/gemm_tc.cu, csrc/tc_api.cuh) with every option the pipelines use:
  * C = epilogue(sum over segments i < nseg of A[:, a_off[i] : +K] . B[:, b_off[i] : +K]^T)   (offsets in fp16 units; f8[i] != 0:
  * the segment holds K e4m3 bytes).  a_off_host / b_off_host / f8_host are HOST int[nseg].  Epilogue, in this order: times
@@ -164,6 +164,39 @@ int sampt_test_sam_upscale(sampt_ctx* ctx, const float* u1, const float* hyper, 
  * n_done (device int) = 1. */
 int sampt_test_sam_postprocess(sampt_ctx* ctx, const float* low_res, int n_masks, int G, int in_h, int in_w, int H, int W, float* out,
                                int* bbox5, float* box4, int* skip, int* n_done, void* stream);
+/* Five stages of the PIPS tracker (csrc/pips_kernels.cu) through the launchers of sampt_pips_fnet / sampt_pips_track, with the
+ * registered "pips.*" weights.  slots_host (HOST int[S] or NULL = 0..S-1) is the frame feeding each window slot, active_host (HOST
+ * uint8[N] or NULL = all) the points taking part; f and n_missing as in the linking of sam_pt/point_tracker/pips/tracker.py:72-148. */
+/* One encoder convolution by weight name ("fnet.conv1", "fnet.layer2.0.conv1", "fnet.conv2", ...): tc != 0 runs im2col + 3-pass
+ * tensor-core GEMM (needs the ".w16" weights), else the fp32 CUDA-core kernel.  "fnet.conv1": in = planar frames (Nimg,3,H,W),
+ * uint8 (is_f32 == 0) or float 0..255, normalised 2*(x/255)-1 on the fly; any other name: in = fp32 NHWC (Nimg,H,W,Cin).
+ * out (Nimg,Ho,Wo,Cout) fp32 NHWC, Ho = (H + 2 pad - R) / stride + 1. */
+int sampt_test_pips_conv(sampt_ctx* ctx, const char* name, int tc, const void* in, int is_f32, int Nimg, int H, int W, int Cin,
+                         int Cout, int R, int stride, int pad, float* out, void* stream);
+/* InstanceNorm2d (eps 1e-5) as ResidualBlock uses it, on x (Nimg,HW,C) NHWC -> y:  mode 0: relu(IN(x));  mode 1: relu(relu(IN(x)) +
+ * res);  mode 2: relu(relu(IN(x)) + IN(res)).  stats / res_stats (Nimg,C,2) receive the (mean, rstd) pairs the kernel applies
+ * (res_stats only in mode 2).  y may alias x. */
+int sampt_test_pips_inorm(sampt_ctx* ctx, const float* x, const float* res, int mode, int Nimg, int HW, int C, float* y, float* stats,
+                          float* res_stats, void* stream);
+/* F.interpolate(bilinear, align_corners=True) of in (Nimg,Hi,Wi,C) into channels [coff, coff + C) of out (Nimg,Ho,Wo,Ctot). */
+int sampt_test_pips_resize(sampt_ctx* ctx, const float* in, int Nimg, int Hi, int Wi, int C, float* out, int Ho, int Wo, int Ctot,
+                           int coff, void* stream);
+/* The fused correlation lookup with the whole mixer row: pyramid levels (frames,H_l,W_l,128), ffeats (N,S,128), coords (N,S,2)
+ * level-0 feature px -> xin (N*S, 520) = [ffeat 128 | corr 196 | sincos(dx,dy,t) 192 | dx,dy,t | 0]; rows of inactive points are
+ * not written. */
+int sampt_test_pips_corr(sampt_ctx* ctx, const float* fmaps, const float* l1, const float* l2, const float* l3, int H4, int W4,
+                         const float* ffeats, const float* coords, int N, int S, const uint8_t* active_host, int f, int n_missing,
+                         const int* slots_host, float* xin, void* stream);
+/* One per-window operation on caller-owned state (S = 8): coords (N,S,2), ffeats (N,S,128), feat_init (N,128), traj (T,N,2),
+ * vis (T,N), cur (N) int32.  op 0 / 1: window init (coords = traj[f] / stride, ffeats = feat_init, or with op 1 bilinear_sample2d
+ * of fmaps (frames,H4,W4,128) at slot 0's frame, stored into feat_init too); 2: token mixing of mixer layer `layer` (0..11) on x
+ * (N,S,512) in place, then the channel-mixing LayerNorm into xln; 3: the final LayerNorm of x into xln; 4: x (N,512) = mean over
+ * S of xln; 5: feature / coordinate update from delta (N, S*130); 6: visibility head, trajectory write-back and linking with
+ * threshold thr0. */
+int sampt_test_pips_window_op(sampt_ctx* ctx, int op, int N, int S, int T, int stride, int f, int n_missing, const int* slots_host,
+                              const uint8_t* active_host, const float* fmaps, int H4, int W4, float* coords, float* ffeats,
+                              float* feat_init, float* traj, float* vis, int* cur, float* x, float* xln, int layer,
+                              const float* delta, float thr0, void* stream);
 
 /* ---- SAM image encoder ------------------------------------------------------------------------------------------ */
 /* ResizeLongestSide.apply_image (PIL bilinear, bit-exact): planar uint8 (B,3,H,W) -> (B,3,Ho,Wo); coefficient tables

@@ -70,10 +70,11 @@ def bilinear_sample2d(im, x, y):
         idx = (yy * W + xx).long()
         return torch.gather(flat, 1, idx[:, :, None].expand(-1, -1, C))
 
-    w00 = ((x1.float() - x) * (y1.float() - y)).unsqueeze(2)
-    w01 = ((x - x0.float()) * (y1.float() - y)).unsqueeze(2)
-    w10 = ((x1.float() - x) * (y - y0.float())).unsqueeze(2)
-    w11 = ((x - x0.float()) * (y - y0.float())).unsqueeze(2)
+    x0f, x1f, y0f, y1f = (t.to(x.dtype) for t in (x0, x1, y0, y1))
+    w00 = ((x1f - x) * (y1f - y)).unsqueeze(2)
+    w01 = ((x - x0f) * (y1f - y)).unsqueeze(2)
+    w10 = ((x1f - x) * (y - y0f)).unsqueeze(2)
+    w11 = ((x - x0f) * (y - y0f)).unsqueeze(2)
     out = w00 * g(y0c, x0c) + w01 * g(y0c, x1c) + w10 * g(y1c, x0c) + w11 * g(y1c, x1c)
     return out.permute(0, 2, 1)
 
@@ -94,29 +95,30 @@ def corr_lookup(pyr: List[torch.Tensor], ffeats, coords, radius: int = 3):
     NB the window is TRANSPOSED (pips.py:378-384): x takes the `dy` grid."""
     B, S, N, C = ffeats.shape
     r = radius
+    dt, dev = ffeats.dtype, ffeats.device
     out = []
     for i, fm in enumerate(pyr):
         H, W = fm.shape[-2:]
         corrs = torch.matmul(ffeats, fm.reshape(B, S, C, H * W)).view(B, S, N, H, W)
-        corrs = corrs / torch.sqrt(torch.tensor(C).float())
-        dx = torch.linspace(-r, r, 2 * r + 1)
-        dy = torch.linspace(-r, r, 2 * r + 1)
+        corrs = corrs / torch.sqrt(torch.tensor(float(C), dtype=dt, device=dev))
+        dx = torch.linspace(-r, r, 2 * r + 1, dtype=dt, device=dev)
+        dy = torch.linspace(-r, r, 2 * r + 1, dtype=dt, device=dev)
         delta = torch.stack(torch.meshgrid(dy, dx, indexing="ij"), dim=-1)
         cl = coords.reshape(B * S * N, 1, 1, 2) / 2 ** i + delta.view(1, 2 * r + 1, 2 * r + 1, 2)
         xg = 2 * cl[..., 0:1] / (W - 1) - 1
         yg = 2 * cl[..., 1:2] / (H - 1) - 1
         samp = F.grid_sample(corrs.reshape(B * S * N, 1, H, W), torch.cat([xg, yg], dim=-1), align_corners=True)
         out.append(samp.view(B, S, N, -1))
-    return torch.cat(out, dim=-1).contiguous().float()
+    return torch.cat(out, dim=-1).contiguous()
 
 
 def get_3d_embedding(xyz, C: int = 64):
     """utils/misc.py:30-55 with cat_coords=True. xyz (B,N,3) -> (B,N,3C+3)."""
-    div = (torch.arange(0, C, 2, dtype=torch.float32) * (1000.0 / C)).reshape(1, 1, C // 2)
+    div = (torch.arange(0, C, 2, dtype=xyz.dtype, device=xyz.device) * (1000.0 / C)).reshape(1, 1, C // 2)
     pes = []
     for d in range(3):
         v = xyz[:, :, d:d + 1]
-        pe = torch.zeros(xyz.shape[0], xyz.shape[1], C)
+        pe = torch.zeros(xyz.shape[0], xyz.shape[1], C, dtype=xyz.dtype, device=xyz.device)
         pe[:, :, 0::2] = torch.sin(v * div)
         pe[:, :, 1::2] = torch.cos(v * div)
         pes.append(pe)
@@ -171,7 +173,7 @@ def pips_forward(sd: SD, xys, rgbs, feat_init=None, iters: int = 6, stride: int 
         LRR = fcorrs.shape[3]
         fcorrs_ = fcorrs.permute(0, 2, 1, 3).reshape(B * N, S, LRR)
         flows_ = (coords - coords[:, 0:1]).permute(0, 2, 1, 3).reshape(B * N, S, 2)
-        times_ = torch.linspace(0, S, S).reshape(1, S, 1).repeat(B * N, 1, 1)
+        times_ = torch.linspace(0, S, S, dtype=coords.dtype, device=coords.device).reshape(1, S, 1).repeat(B * N, 1, 1)
         flows_ = torch.cat([flows_, times_], dim=2)
         ffeats_ = ffeats.permute(0, 2, 1, 3).reshape(B * N, S, LATENT)
         delta = delta_block(sd, ffeats_, fcorrs_, flows_, S)
@@ -197,18 +199,20 @@ def pips_forward(sd: SD, xys, rgbs, feat_init=None, iters: int = 6, stride: int 
 def track_one_direction(sd: SD, rgbs, query_points, s: int = 8, stride: int = 4, thr0: float = 0.9,
                         fmaps_all: Optional[torch.Tensor] = None, log: Optional[list] = None):
     """pips/tracker.py:42-153.  rgbs (1,T,3,H,W) any dtype; query_points (1,N,3).
-    `fmaps_all` (T,128,H/4,W/4): per-frame encoder features computed once (results-neutral shortcut)."""
+    `fmaps_all` (T,128,H/4,W/4): per-frame encoder features computed once (results-neutral shortcut).
+    Runs in the dtype and on the device of `query_points`."""
     B, T = rgbs.shape[:2]
     N = query_points.shape[1]
     if B != 1:
         raise NotImplementedError("Batch size > 1 is not supported for PIPS yet")
-    traj = torch.zeros((T, N, 2))
-    vis = torch.zeros((T, N))
+    dt, dev = query_points.dtype, query_points.device
+    traj = torch.zeros((T, N, 2), dtype=dt, device=dev)
+    vis = torch.zeros((T, N), dtype=dt, device=dev)
     start = query_points[0, :, 0].long()
-    ar = torch.arange(N)
+    ar = torch.arange(N, device=dev)
     vis[start, ar] = 1.0
     traj[start, ar, :] = query_points[0, :, 1:]
-    feat_init = torch.zeros((1, N, LATENT))
+    feat_init = torch.zeros((1, N, LATENT), dtype=dt, device=dev)
     cur = start.clone()
     for f in range(T - 1):
         if (cur == f).sum() == 0:
@@ -220,22 +224,22 @@ def track_one_direction(sd: SD, rgbs, query_points, s: int = 8, stride: int = 4,
             rg = None
         else:
             fm = None
-            rg = rgbs[:, idx].float()
+            rg = rgbs[:, idx].to(dt)
         born = start == f
         if born.any():
             _, _, ff = pips_forward(sd, traj[None, f, born, :], rg, None, 6, stride, s, fmaps=fm)
             feat_init[:, born, :] = ff
         act = cur == f
         preds, vis_e, _ = pips_forward(sd, traj[None, f, act, :], rg, feat_init[:, act, :], 6, stride, s, fmaps=fm)
-        out_vis = torch.sigmoid(vis_e).float()
-        out_traj = preds[-1].float()
+        out_vis = torch.sigmoid(vis_e)
+        out_traj = preds[-1]
         if log is not None:
             log.append({"frame": f, "active": act.clone(), "traj": out_traj.clone(), "vis": out_vis.clone()})
         osl = slice(1, s - n_missing)
         psl = slice(1 + f, f + s - n_missing)
         vis[psl, act] = out_vis[0, osl, :]
         traj[psl, act, :] = out_traj[0, osl, :, :]
-        thr = torch.where(act, torch.ones(N) * thr0, torch.zeros(N))
+        thr = torch.where(act, torch.ones(N, dtype=dt, device=dev) * thr0, torch.zeros(N, dtype=dt, device=dev))
         earliest = torch.where(act, cur + 1, cur)
         last = torch.where(act, cur + s - n_missing - 1, cur)
         nxt = last

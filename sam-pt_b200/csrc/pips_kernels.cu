@@ -300,11 +300,16 @@ int im2col_conv1_split(Ctx* c, cudaStream_t st, const void* frames, int is_f32, 
 }
 
 // InstanceNorm2d (no affine, eps 1e-5, biased variance; pips.py:207-209), channels-last.
-// pass 1: per (image, row-chunk) partial sum / sum of squares per channel.
+// pass 1 sums d = x - xc and d^2 per (image, row-chunk) and channel, xc = the channel's pixel at the centre of the image (index
+// HW/2).  The shift keeps E[d^2] - E[d]^2 well conditioned when the mean is large against the spread (a nearly constant channel with
+// an O(1) conv bias, as black or letterboxed frames produce): from sums of x and x^2 the fp32 rounding would cost a relative
+// variance error ~ u (mean/std)^2.  Where xc is far from the mean on the scale of the spread (mean - xc)^2 > 8 (var + eps),
+// pass 2 sums d = x - mean instead and replaces that channel's statistics.
+// shift = null: pass 1; else pass 2, shift[(img*C + c)*2] = the mean of pass 1.
 // 256 threads = (C/4 float4 channel lanes) x (256/(C/4) pixel rows): 16-byte coalesced loads, `rows` pixels in flight per lane
-// group, fp32 partial sums over <= chunk/rows pixels promoted to fp64 before the cross-row / cross-chunk reduction.
+// group, fp32 partial sums over <= 64 pixels promoted to fp64 before the cross-row / cross-chunk reduction.
 __global__ void __launch_bounds__(256)
-inorm_partial_kernel(const float* __restrict__ x, double* __restrict__ part, int HW, int C, int chunk) {
+inorm_partial_kernel(const float* __restrict__ x, const float* __restrict__ shift, double* __restrict__ part, int HW, int C, int chunk) {
   const int img = blockIdx.z, ch = blockIdx.y;
   const int c4n = C >> 2, rows = 256 / c4n;
   const int lane4 = threadIdx.x % c4n, row = threadIdx.x / c4n;
@@ -314,10 +319,18 @@ inorm_partial_kernel(const float* __restrict__ x, double* __restrict__ part, int
   double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   if (row < rows) {
     const float* base = x + (size_t)img * HW * C + lane4 * 4;
+    float4 x0;
+    if (shift) {
+      const float* sp = shift + ((size_t)img * C + lane4 * 4) * 2;
+      x0 = make_float4(sp[0], sp[2], sp[4], sp[6]);
+    } else {
+      x0 = *reinterpret_cast<const float4*>(base + (size_t)(HW / 2) * C);
+    }
     int cnt = 0;
 #pragma unroll 4
     for (int p = p0 + row; p < p1; p += rows) {
-      const float4 v = *reinterpret_cast<const float4*>(base + (size_t)p * C);
+      float4 v = *reinterpret_cast<const float4*>(base + (size_t)p * C);
+      v.x -= x0.x; v.y -= x0.y; v.z -= x0.z; v.w -= x0.w;
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
       ss.x = fmaf(v.x, v.x, ss.x); ss.y = fmaf(v.y, v.y, ss.y); ss.z = fmaf(v.z, v.z, ss.z); ss.w = fmaf(v.w, v.w, ss.w);
       if (++cnt == 64) {
@@ -339,8 +352,10 @@ inorm_partial_kernel(const float* __restrict__ x, double* __restrict__ part, int
     for (int k = 0; k < 8; ++k) o[k] = acc[k];  // [c][sum, sumsq] for the 4 channels of this lane
   }
 }
-__global__ void inorm_final_kernel(const double* __restrict__ part, float* __restrict__ stats, int nchunks, int C, int HW,
-                                   float eps) {
+// stats[(img*C + c)*2 + {0,1}] = (mean, rstd); shift as in inorm_partial_kernel (it may alias stats: each thread reads its own
+// channel's shift before writing it)
+__global__ void inorm_final_kernel(const float* __restrict__ x, const float* shift, const double* __restrict__ part, float* stats,
+                                   int nchunks, int C, int HW, float eps) {
   const int img = blockIdx.y;
   const int cidx = blockIdx.x * blockDim.x + threadIdx.x;
   if (cidx >= C) return;
@@ -350,10 +365,14 @@ __global__ void inorm_final_kernel(const double* __restrict__ part, float* __res
     s += part[o];
     ss += part[o + 1];
   }
-  double mean = s / HW;
-  double var = ss / HW - mean * mean;
+  const double dmean = s / HW;   // mean of d
+  double var = ss / HW - dmean * dmean;
   if (var < 0) var = 0;
-  stats[((size_t)img * C + cidx) * 2] = (float)mean;
+  const double xc = (double)x[((size_t)img * HW + HW / 2) * C + cidx];
+  const double x0 = shift ? (double)shift[((size_t)img * C + cidx) * 2] : xc;
+  // pass 2 keeps pass 1's statistics where they are as accurate (relative variance error gamma_64 (1 + (mean - xc)^2 / var))
+  if (shift && (x0 - xc) * (x0 - xc) <= 8.0 * (var + (double)eps)) return;
+  stats[((size_t)img * C + cidx) * 2] = (float)(x0 + dmean);
   stats[((size_t)img * C + cidx) * 2 + 1] = (float)(1.0 / sqrt(var + (double)eps));
 }
 // pass 2: y = relu?( (x-mean)*rstd [+ res] ).  res_stats != null -> residual is itself instance-normed first
@@ -397,12 +416,16 @@ int inorm_stats(Ctx* c, cudaStream_t st, const float* x, float* stats, double* p
   int nchunks = cdiv(HW, chunk);
   SAMPT_CHECK(C % 4 == 0 && C <= 1024, "inorm_stats: unsupported channel count %d", C);
   dim3 g1(1, nchunks, Nimg);
-  inorm_partial_kernel<<<g1, 256, 0, st>>>(x, part, HW, C, chunk);
-  SAMPT_LAUNCH_CHECK();
   dim3 g2(cdiv(C, 64), Nimg);
-  inorm_final_kernel<<<g2, 64, 0, st>>>(part, stats, nchunks, C, HW, 1e-5f);
+  inorm_partial_kernel<<<g1, 256, 0, st>>>(x, nullptr, part, HW, C, chunk);   // shifted by the centre pixel
   SAMPT_LAUNCH_CHECK();
-  c->launches += 2;
+  inorm_final_kernel<<<g2, 64, 0, st>>>(x, nullptr, part, stats, nchunks, C, HW, 1e-5f);
+  SAMPT_LAUNCH_CHECK();
+  inorm_partial_kernel<<<g1, 256, 0, st>>>(x, stats, part, HW, C, chunk);     // centred on pass 1's mean
+  SAMPT_LAUNCH_CHECK();
+  inorm_final_kernel<<<g2, 64, 0, st>>>(x, stats, part, stats, nchunks, C, HW, 1e-5f);
+  SAMPT_LAUNCH_CHECK();
+  c->launches += 4;
   return 0;
 }
 int inorm_apply(Ctx* c, cudaStream_t st, const float* x, const float* stats, const float* res, const float* res_stats,
@@ -571,9 +594,13 @@ pips_corr_kernel(PipsWin w, float* __restrict__ xin, int ldx) {
   if (threadIdx.x == 0) {
     sflow[0] = cx0 - w.coords[((size_t)n * w.S + 0) * 2 + 0];
     sflow[1] = cy0 - w.coords[((size_t)n * w.S + 0) * 2 + 1];
-    // times_ = linspace(0, S, S)  (pips.py:527): step = S/(S-1)
-    sflow[2] = (w.S > 1) ? (float)s * ((float)w.S / (float)(w.S - 1)) : 0.f;
-    if (s == w.S - 1) sflow[2] = (float)w.S;
+    // times_ = linspace(0, S, S)  (pips.py:527) with torch's two-sided rule: step = S/(S-1); slots below S/2 are s * step, the
+    // others S - step * (S-1-s), each product and difference rounded on its own (no fma contraction)
+    if (w.S <= 1) sflow[2] = 0.f;
+    else {
+      const float step = (float)w.S / (float)(w.S - 1);
+      sflow[2] = (s < w.S / 2) ? __fmul_rn((float)s, step) : __fsub_rn((float)w.S, __fmul_rn(step, (float)(w.S - 1 - s)));
+    }
   }
   __syncthreads();
   float* row = xin + ((size_t)n * w.S + s) * ldx;

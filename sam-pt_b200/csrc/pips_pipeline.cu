@@ -31,7 +31,7 @@ static bool fnet_uses_tc(const Ctx* c, const std::string& prefix) {
 // c->fnet_prefix: weight-name prefix of the encoder being run ("pips." or "cot."; the CoTracker BasicEncoder has the same
 // architecture).  Both live in the ctx (not process-wide) so that encoders of different ctxs / devices never see each other's.
 
-static int conv_by_name(Ctx* c, cudaStream_t st, const std::string& name, const Act& in, Act* out, int R, int stride, int pad) {
+int conv_by_name(Ctx* c, cudaStream_t st, const std::string& name, const Act& in, Act* out, int R, int stride, int pad) {
   if (c->fnet_im2col != nullptr) {
     // implicit-GEMM on tensor cores: A = im2col(in) as fp16 hi|lo, B = weights hi|lo, 3 split passes (~fp32), fp32 NHWC output
     const __half* w16; const float* b;
@@ -49,6 +49,26 @@ static int conv_by_name(Ctx* c, cudaStream_t st, const std::string& name, const 
   SAMPT_TRY(get_f32(c, c->fnet_prefix + name + ".weight_rsck", &w));
   SAMPT_TRY(get_f32(c, c->fnet_prefix + name + ".bias", &b));
   return conv_nhwc_f32(c, st, in.p, w, b, out->p, in.n, in.h, in.w, in.c, out->c, R, R, stride, pad);
+}
+
+// conv1 (7x7 stride 2 pad 3, 3 -> 64) on planar frames (uint8, or float holding 0..255), normalisation 2*(x/255)-1 fused:
+// im2col + 3-pass tensor-core GEMM when c->fnet_im2col is set, else the fp32 CUDA-core kernel.  out: (n, H2, W2, 64) channels-last.
+int conv1_frames(Ctx* c, cudaStream_t st, const void* frames, int is_f32, int n, int H, int W, float* out) {
+  const int H2 = (H + 6 - 7) / 2 + 1, W2 = (W + 6 - 7) / 2 + 1;
+  if (c->fnet_im2col != nullptr) {
+    const __half* w16; const float* b1;
+    SAMPT_TRY(get_f16(c, c->fnet_prefix + "fnet.conv1.w16", &w16));
+    SAMPT_TRY(get_f32(c, c->fnet_prefix + "fnet.conv1.bias", &b1));
+    SAMPT_TRY(im2col_conv1_split(c, st, frames, is_f32, c->fnet_im2col, n, H, W, 192));
+    GemmSeg seg{3, {0, 192, 0}, {0, 0, 192}};
+    GemmEpi ep{};
+    ep.out32 = out; ep.bias = b1; ep.ldc = 64;
+    return gemm_tc(c, st, c->fnet_im2col, 384, w16, 384, n * H2 * W2, 64, 192, seg, ep);
+  }
+  const float *w1, *b1;
+  SAMPT_TRY(get_f32(c, c->fnet_prefix + "fnet.conv1.weight_rsck", &w1));
+  SAMPT_TRY(get_f32(c, c->fnet_prefix + "fnet.conv1.bias", &b1));
+  return conv7x7s2(c, st, frames, is_f32, w1, b1, out, n, H, W);
 }
 
 // ResidualBlock (pips.py:139-188): y = relu(IN(conv1 x)); y = relu(IN(conv2 y)); x' = IN(conv1x1 x) if stride>1; relu(x'+y)
@@ -98,20 +118,8 @@ static int fnet_chunk(Ctx* c, cudaStream_t st, const void* frames, int is_f32, i
     // largest im2col operand: max(layer1: H2*W2 x 2*576, conv2: Ho*Wo x 2*3776) halves per frame
     size_t a_elems = std::max((size_t)H2 * W2 * 2 * 576, (size_t)Ho * Wo * 2 * 3776) * n;
     SAMPT_TRY(ws_get(c, &c->fnet_im2col, a_elems, "fnet im2col operand"));
-    const __half* w16; const float* b1;
-    SAMPT_TRY(get_f16(c, c->fnet_prefix + "fnet.conv1.w16", &w16));
-    SAMPT_TRY(get_f32(c, c->fnet_prefix + "fnet.conv1.bias", &b1));
-    SAMPT_TRY(im2col_conv1_split(c, st, frames, is_f32, c->fnet_im2col, n, H, W, 192));
-    GemmSeg seg{3, {0, 192, 0}, {0, 0, 192}};
-    GemmEpi ep{};
-    ep.out32 = x.p; ep.bias = b1; ep.ldc = 64;
-    SAMPT_TRY(gemm_tc(c, st, c->fnet_im2col, 384, w16, 384, n * H2 * W2, 64, 192, seg, ep));
-  } else {
-    const float *w1, *b1;
-    SAMPT_TRY(get_f32(c, c->fnet_prefix + "fnet.conv1.weight_rsck", &w1));
-    SAMPT_TRY(get_f32(c, c->fnet_prefix + "fnet.conv1.bias", &b1));
-    SAMPT_TRY(conv7x7s2(c, st, frames, is_f32, w1, b1, x.p, n, H, W));
   }
+  SAMPT_TRY(conv1_frames(c, st, frames, is_f32, n, H, W, x.p));
   SAMPT_TRY(inorm_stats(c, st, x.p, s.stats_a, s.part, n, H2 * W2, 64));
   SAMPT_TRY(inorm_apply(c, st, x.p, s.stats_a, nullptr, nullptr, x.p, n, H2 * W2, 64, 1, 0));
 
@@ -541,4 +549,143 @@ extern "C" int sampt_pips_corr_lookup(sampt_ctx* ctx, const float* fmaps, const 
   SAMPT_CUDA(cudaMemcpy2DAsync(fcorr, 196 * sizeof(float), xin + 128, 520 * sizeof(float), 196 * sizeof(float), (size_t)N * S,
                                cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+// ---- unit-test entries: one tracker stage on caller buffers, through the same launchers as the encoder and the window chain --------
+static const int* test_window_params(Ctx* c, cudaStream_t st, int f, int n_missing, const int* slots_host, int S) {
+  int* wp_d;
+  if (ws_get(c, &wp_d, 16, "window params") != 0) return nullptr;
+  int* wp_h = reinterpret_cast<int*>(reinterpret_cast<char*>(c->pinned) + (64 << 10));
+  wp_h[0] = f; wp_h[1] = n_missing;
+  for (int s = 0; s < 8; ++s) wp_h[2 + s] = (slots_host && s < S) ? slots_host[s] : s;
+  if (cudaMemcpyAsync(wp_d, wp_h, 10 * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+      cudaStreamSynchronize(st) != cudaSuccess) {   // the pinned staging slot is reused by the next call
+    set_error("test window params: copy failed");
+    return nullptr;
+  }
+  return wp_d;
+}
+
+static int test_active(Ctx* c, cudaStream_t st, const uint8_t* active_host, int N, uint8_t** out) {
+  SAMPT_TRY(ws_get(c, out, (size_t)N, "active"));
+  if (active_host) SAMPT_CUDA(cudaMemcpyAsync(*out, active_host, (size_t)N, cudaMemcpyHostToDevice, st));
+  else SAMPT_CUDA(cudaMemsetAsync(*out, 1, (size_t)N, st));
+  SAMPT_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+extern "C" int sampt_test_pips_conv(sampt_ctx* ctx, const char* name, int tc, const void* in, int is_f32, int Nimg, int H, int W,
+                                    int Cin, int Cout, int R, int stride, int pad, float* out, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const std::string nm(name);
+  c->ws_reset();
+  c->fnet_prefix = "pips.";
+  c->fnet_im2col = nullptr;
+  const int Ho = (H + 2 * pad - R) / stride + 1, Wo = (W + 2 * pad - R) / stride + 1;
+  if (tc) {
+    const int Kp = nm == "fnet.conv1" ? 192 : ((R * R * Cin + 63) / 64) * 64;
+    SAMPT_TRY(ws_get(c, &c->fnet_im2col, (size_t)Nimg * Ho * Wo * 2 * Kp, "fnet im2col operand"));
+  }
+  int rc;
+  if (nm == "fnet.conv1") {
+    SAMPT_CHECK(Cin == 3 && Cout == 64 && R == 7 && stride == 2 && pad == 3, "sampt_test_pips_conv: conv1 is 7x7 s2 p3, 3 -> 64");
+    rc = conv1_frames(c, st, in, is_f32, Nimg, H, W, out);
+  } else {
+    SAMPT_CHECK(is_f32, "sampt_test_pips_conv: %s takes fp32 NHWC input", name);
+    Act a{const_cast<float*>(static_cast<const float*>(in)), Nimg, H, W, Cin};
+    Act o{out, Nimg, Ho, Wo, Cout};
+    rc = conv_by_name(c, st, nm, a, &o, R, stride, pad);
+  }
+  c->fnet_im2col = nullptr;
+  return rc;
+}
+
+extern "C" int sampt_test_pips_inorm(sampt_ctx* ctx, const float* x, const float* res, int mode, int Nimg, int HW, int C, float* y,
+                                     float* stats, float* res_stats, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(mode >= 0 && mode <= 2, "sampt_test_pips_inorm: unknown mode %d", mode);
+  SAMPT_CHECK(mode == 0 || res != nullptr, "sampt_test_pips_inorm: mode %d needs a residual", mode);
+  c->ws_reset();
+  double* part;
+  SAMPT_TRY(ws_get(c, &part, (size_t)Nimg * cdiv(HW, 512) * C * 2, "inorm partials"));
+  SAMPT_TRY(inorm_stats(c, st, x, stats, part, Nimg, HW, C));
+  if (mode == 0) return inorm_apply(c, st, x, stats, nullptr, nullptr, y, Nimg, HW, C, 1, 0);
+  if (mode == 1) return inorm_apply(c, st, x, stats, res, nullptr, y, Nimg, HW, C, 1, 1);
+  SAMPT_TRY(inorm_stats(c, st, res, res_stats, part, Nimg, HW, C));
+  return inorm_apply(c, st, x, stats, res, res_stats, y, Nimg, HW, C, 1, 1);
+}
+
+extern "C" int sampt_test_pips_resize(sampt_ctx* ctx, const float* in, int Nimg, int Hi, int Wi, int C, float* out, int Ho, int Wo,
+                                      int Ctot, int coff, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  SAMPT_CHECK(C % 4 == 0 && Ctot % 4 == 0 && coff % 4 == 0 && coff + C <= Ctot, "sampt_test_pips_resize: bad channel slice");
+  return resize_ac_concat(c, reinterpret_cast<cudaStream_t>(stream), in, out, Nimg, Hi, Wi, C, Ho, Wo, Ctot, coff);
+}
+
+extern "C" int sampt_test_pips_corr(sampt_ctx* ctx, const float* fmaps, const float* l1, const float* l2, const float* l3, int H4, int W4,
+                                    const float* ffeats, const float* coords, int N, int S, const uint8_t* active_host, int f,
+                                    int n_missing, const int* slots_host, float* xin, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(S >= 1 && S <= 8 && N >= 1, "sampt_test_pips_corr: S must be in [1,8], N positive");
+  c->ws_reset();
+  PipsWin w{};
+  w.N = N; w.S = S; w.stride = 4; w.T = S;
+  w.pyr[0] = fmaps; w.pyr[1] = l1; w.pyr[2] = l2; w.pyr[3] = l3;
+  w.H[0] = H4; w.W[0] = W4;
+  for (int l = 1; l < 4; ++l) { w.H[l] = w.H[l - 1] / 2; w.W[l] = w.W[l - 1] / 2; }
+  w.coords = const_cast<float*>(coords);
+  w.ffeats = const_cast<float*>(ffeats);
+  w.wp = test_window_params(c, st, f, n_missing, slots_host, S);
+  if (w.wp == nullptr) return -1;
+  uint8_t* active_d;
+  SAMPT_TRY(test_active(c, st, active_host, N, &active_d));
+  w.active = active_d;
+  return pips_corr(c, st, w, xin, 520);
+}
+
+extern "C" int sampt_test_pips_window_op(sampt_ctx* ctx, int op, int N, int S, int T, int stride, int f, int n_missing,
+                                         const int* slots_host, const uint8_t* active_host, const float* fmaps, int H4, int W4,
+                                         float* coords, float* ffeats, float* feat_init, float* traj, float* vis, int* cur, float* x,
+                                         float* xln, int layer, const float* delta, float thr0, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(N >= 1 && S == 8, "sampt_test_pips_window_op: N positive and S == 8 required");
+  c->ws_reset();
+  MixerW m;
+  SAMPT_TRY(load_mixer(c, &m));
+  PipsWin w{};
+  w.N = N; w.S = S; w.stride = stride; w.T = T;
+  w.pyr[0] = fmaps; w.H[0] = H4; w.W[0] = W4;
+  w.coords = coords; w.ffeats = ffeats; w.feat_init = feat_init; w.traj = traj; w.vis = vis; w.cur = cur;
+  w.wp = test_window_params(c, st, f, n_missing, slots_host, S);
+  if (w.wp == nullptr) return -1;
+  uint8_t* active_d;
+  SAMPT_TRY(test_active(c, st, active_host, N, &active_d));
+  w.active = active_d;
+  switch (op) {
+    case 0:
+    case 1:
+      w.sample_feat = op;
+      return pips_window_init(c, st, w);
+    case 2: {
+      SAMPT_CHECK(layer >= 0 && layer < 12, "sampt_test_pips_window_op: layer %d out of [0, 12)", layer);
+      const int l = layer;
+      return mixer_token(c, st, x, xln, w.active, N, m.ln0_w[l], m.ln0_b[l], m.tw1[l], m.tb1[l], m.tw2[l], m.tb2[l], m.ln1_w[l],
+                         m.ln1_b[l], 1);
+    }
+    case 3:
+      return mixer_token(c, st, x, xln, w.active, N, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, m.lnf_w, m.lnf_b, 0);
+    case 4:
+      return mixer_mean(c, st, xln, x, N, S, 512);
+    case 5:
+      return pips_update(c, st, w, delta, m.gn_w, m.gn_b, m.up_w, m.up_b);
+    case 6:
+      return pips_link(c, st, w, m.vis_w, m.vis_b, thr0, T);
+    default:
+      set_error("sampt_test_pips_window_op: unknown op %d", op);
+      return -2;
+  }
 }
