@@ -245,6 +245,38 @@ int sampt_vit_encode_f32(sampt_ctx* ctx, const float* x, int B, int depth, int e
  * called whenever the image-encoder weights are re-registered.  A no-op when that path is off. */
 int sampt_vit_cache_clear(sampt_ctx* ctx);
 
+/* ---- TinyViT image encoder of MobileSAM / Light HQ-SAM (csrc/tinyvit.cu) ------------------------------------------------
+ * Upstream mobile_sam/modeling/tiny_vit_sam.py (TinyViT.forward) and sam-hq's copy of it, configuration of
+ * configs/model/sam/sam_mobile_vit_tiny.yaml / samhq_light_vit_tiny.yaml (embed_dims 64/128/160/320, depths 2/2/6/2,
+ * heads 2/4/5/10, windows 7/7/14/7).  Weights are registered under "sam.tinyvit." (BatchNorm folded, layouts in
+ * sam-pt_b200/mobile_sam/modeling/tiny_vit_sam.py).  Work buffers come from the ViT slab (sampt_ctx_set_vit_workspace), whose size
+ * for B frames sampt_tinyvit_workspace_bytes returns.
+ * sampt_tinyvit_encode replaces SamPredictor.set_image's encoder call (sam_pt.py:849) for these models:
+ *   is_f32 = 0: image = resized uint8 frames (B,3,Hr,Wr); Sam.preprocess (normalise with the HOST mean3 / std3, zero-pad
+ *               to 1024^2) is fused into the stem's im2col;
+ *   is_f32 = 1: image = upstream forward's preprocessed (B,3,1024,1024) float image (Hr, Wr, mean3, std3 unused).
+ * feats (B,256,64,64) fp32; interm (B,64,64,160) or NULL: layers.1's output, sam-hq's interm_embeddings[0]. */
+int sampt_tinyvit_workspace_bytes(int B, size_t* out);
+int sampt_tinyvit_encode(sampt_ctx* ctx, const void* image, int is_f32, int B, int Hr, int Wr, const float* mean3,
+                         const float* std3, float* feats, float* interm, void* stream);
+/* Unit-test entries; each calls the launchers of sampt_tinyvit_encode.
+ * stem: patch_embed.seq (TinyViT.patch_embed) -> out (B,256,256,64) token-major.
+ * dwconv: one depthwise Conv2d_BN 3x3 (pad 1, stride 1|2, optional GELU) over x (B,H,W,C), w [9][C] tap-major, bias [C]
+ *   -> out32 (B*Ho*Wo, C) and / or out16 (B*Ho*Wo, 2*Kp) fp16 hi|lo with zero columns [C, Kp).
+ * block_attn: TinyViTBlock.forward's first half, x + attn(window_partition(pad(x))), of layers.<stage>.blocks.<blk> on x
+ *   (B,H,H,C); qkv_out (B*H*H [+1], 3C) receives the qkv GEMM output (the LN(0) row last when the map is padded), attn_out
+ *   (B*H*H, 2*pad64(C)) halves the proj GEMM's operand; both optional.
+ * stage: layers.<stage> including its PatchMerging, x (B, R*R, C) -> out at the next stage's resolution and width.
+ * neck: x (B, 4096, 320) -> feats (B,256,64,64). */
+int sampt_test_tinyvit_stem(sampt_ctx* ctx, const void* image, int is_f32, int B, int Hr, int Wr, const float* mean3,
+                            const float* std3, float* out, void* stream);
+int sampt_test_tinyvit_dwconv(sampt_ctx* ctx, const float* x, const float* w, const float* bias, int B, int H, int W, int C,
+                              int stride, int act, float* out32, void* out16, int Kp, void* stream);
+int sampt_test_tinyvit_block_attn(sampt_ctx* ctx, int stage, int blk, const float* x, int B, int H, float* out, float* qkv_out,
+                                  void* attn_out, void* stream);
+int sampt_test_tinyvit_stage(sampt_ctx* ctx, int stage, const float* x, int B, float* out, void* stream);
+int sampt_test_tinyvit_neck(sampt_ctx* ctx, const float* x, int B, float* feats, void* stream);
+
 /* HQ-SAM (segment_anything_hq.modeling.mask_decoder_hq.MaskDecoderHQ, un-vendored m43/sam-hq @ 75c73fa; config
  * configs/model/sam/samhq_vit_huge.yaml:19-27).  sampt_sam_hq_features computes the per-frame
  * `embedding_encoder(image_embeddings) + compress_vit_feat(interm_embeddings[0])` map ([16*G*G][32], channels-last);

@@ -101,6 +101,18 @@ struct Ctx {
   }
 };
 
+// For its lifetime, points the ctx's bump allocator at the image-encoder slab (sampt_ctx_set_vit_workspace) when one is
+// registered, from offset 0; the general workspace is restored on exit.  The ViT and TinyViT encoders allocate through it so
+// that they can run on their own stream next to the PIPS / decode pipelines.
+struct VitSlabGuard {
+  Ctx* c; char* b; size_t n, o; bool on;
+  explicit VitSlabGuard(Ctx* c_) : c(c_), b(c_->ws_base), n(c_->ws_bytes), o(c_->ws_off), on(c_->vit_base != nullptr) {
+    if (on) { c->ws_base = c->vit_base; c->ws_bytes = c->vit_bytes; }
+    c->ws_off = 0;
+  }
+  ~VitSlabGuard() { if (on) { c->ws_base = b; c->ws_bytes = n; c->ws_off = o; } }
+};
+
 template <typename T>
 inline int ws_get(Ctx* c, T** out, size_t count, const char* what) {
   *out = reinterpret_cast<T*>(c->ws_alloc(count * sizeof(T)));

@@ -123,14 +123,7 @@ static int vit_forward(Ctx* c, cudaStream_t st, const uint8_t* img, const float*
   const int Kpe = 3 * d.P * d.P;
   const std::string p = "sam.image_encoder.";
   // the encoder allocates from its own slab when one is registered (stream-level overlap with PIPS / decode)
-  struct SlabGuard {
-    Ctx* c; char* b; size_t n, o; bool on;
-    SlabGuard(Ctx* c_) : c(c_), b(c_->ws_base), n(c_->ws_bytes), o(c_->ws_off), on(c_->vit_base != nullptr) {
-      if (on) { c->ws_base = c->vit_base; c->ws_bytes = c->vit_bytes; }
-      c->ws_off = 0;
-    }
-    ~SlabGuard() { if (on) { c->ws_base = b; c->ws_bytes = n; c->ws_off = o; } }
-  } slab_guard(c);
+  VitSlabGuard slab_guard(c);
 
   float* x;           SAMPT_TRY(ws_get(c, &x, (size_t)Mtok * D, "vit x"));
   __half* A;          SAMPT_TRY(ws_get(c, &A, (size_t)std::max(Mwin, Mtok) * std::max(D, Kpe) * asp, "vit A"));

@@ -36,5 +36,12 @@ def __getattr__(name):
         globals()["SamHQHydra"] = SamHQHydra
         return SamHQHydra
     if name == "MobileSamHydra":
-        raise ImportError("MobileSAM is outside the H100 hot-path scope (SURVEY §2 row 2)")
+        from mobile_sam.modeling import Sam as MobileSam
+
+        class MobileSamHydra(BaseHydra, MobileSam):
+            def __init__(self, *args, **kwargs):
+                super().__init__(MobileSam, *args, **kwargs)
+
+        globals()["MobileSamHydra"] = MobileSamHydra
+        return MobileSamHydra
     raise AttributeError(name)

@@ -18,9 +18,17 @@ VIT_CFGS = {
     "vit_test": dict(depth=4, embed_dim=128, num_heads=2, global_attn_indexes=[1, 3]),
     "vit_test80": dict(depth=2, embed_dim=640, num_heads=8, global_attn_indexes=[1]),
 }
+# configs/model/sam/sam_mobile_vit_tiny.yaml / samhq_light_vit_tiny.yaml: TinyViT-5M (MobileSAM; Light HQ-SAM with vit_dim 160)
+TINY_VIT = "vit_t"
+TINY_VIT_CFG = dict(img_size=1024, in_chans=3, num_classes=1000, embed_dims=[64, 128, 160, 320], depths=[2, 2, 6, 2],
+                    num_heads=[2, 4, 5, 10], window_sizes=[7, 7, 14, 7], mlp_ratio=4.0, drop_rate=0.0, drop_path_rate=0.0,
+                    use_checkpoint=False, mbconv_expand_ratio=4.0, local_conv_size=3, layer_lr_decay=0.8)
 
 
 def build_sam(vit: str = "vit_b", sam_state_dict: Optional[Dict[str, torch.Tensor]] = None, hq: bool = False):
+    """vit: a VIT_CFGS key, or TINY_VIT for MobileSAM (hq=False) / Light HQ-SAM (hq=True)."""
+    if vit == TINY_VIT:
+        return _build_tiny_sam(sam_state_dict, hq)
     from sam_pt.modeling.sam import SamHydra
     from segment_anything.modeling.image_encoder import ImageEncoderViT
     from segment_anything.modeling.mask_decoder import MaskDecoder
@@ -46,6 +54,32 @@ def build_sam(vit: str = "vit_b", sam_state_dict: Optional[Dict[str, torch.Tenso
     sam = (SamHQHydra if hq else SamHydra)(image_encoder=enc, prompt_encoder=pe, mask_decoder=md, pixel_mean=[123.675, 116.28, 103.53],
                    pixel_std=[58.395, 57.12, 57.375], checkpoint=None, prompt_embed_dim=256, image_size=1024, vit_patch_size=16,
                    image_embedding_size=64)
+    if sam_state_dict is not None:
+        missing, unexpected = sam.load_state_dict(sam_state_dict, strict=False)
+        assert not unexpected, unexpected
+        assert not missing, missing
+    return sam
+
+
+def _build_tiny_sam(sam_state_dict, hq: bool):
+    from segment_anything.modeling.prompt_encoder import PromptEncoder
+    from segment_anything.modeling.transformer import TwoWayTransformer
+    pe = PromptEncoder(embed_dim=256, image_embedding_size=(64, 64), input_image_size=(1024, 1024), mask_in_chans=16)
+    tw = TwoWayTransformer(depth=2, embedding_dim=256, mlp_dim=2048, num_heads=8)
+    if hq:
+        from sam_pt.modeling.sam import SamHQHydra as Hydra
+        from segment_anything_hq.modeling.mask_decoder_hq import MaskDecoderHQ
+        from segment_anything_hq.modeling.tiny_vit_sam import TinyViT
+        md = MaskDecoderHQ(num_multimask_outputs=3, transformer=tw, transformer_dim=256, iou_head_depth=3, iou_head_hidden_dim=256,
+                           vit_dim=160)
+    else:
+        from mobile_sam.modeling.mask_decoder import MaskDecoder
+        from mobile_sam.modeling.tiny_vit_sam import TinyViT
+        from sam_pt.modeling.sam import MobileSamHydra as Hydra
+        md = MaskDecoder(num_multimask_outputs=3, transformer=tw, transformer_dim=256, iou_head_depth=3, iou_head_hidden_dim=256)
+    sam = Hydra(image_encoder=TinyViT(**TINY_VIT_CFG), prompt_encoder=pe, mask_decoder=md, pixel_mean=[123.675, 116.28, 103.53],
+                pixel_std=[58.395, 57.12, 57.375], checkpoint=None, prompt_embed_dim=256, image_size=1024, vit_patch_size=16,
+                image_embedding_size=64)
     if sam_state_dict is not None:
         missing, unexpected = sam.load_state_dict(sam_state_dict, strict=False)
         assert not unexpected, unexpected

@@ -131,6 +131,33 @@ def make_state_dict(shapes: Dict[str, Tuple[int, ...]], seed: int) -> Dict[str, 
     return {k: _init_like_torch(k, tuple(shapes[k]), gen).float().contiguous() for k in sorted(shapes)}
 
 
+def make_tinyvit_state_dict(seed: int, num_classes: int = 1000) -> Dict[str, torch.Tensor]:
+    """TinyViT-5M state dict under upstream key names (mobile_sam/modeling/tiny_vit_sam.py), BatchNorm buffers included.
+    Convs / linears as `_init_like_torch`; BatchNorm: weight U(0.5, 1.5), bias and running_mean U(-0.1, 0.1), running_var
+    U(0.5, 2) (positive, so the folded scale stays O(1)), num_batches_tracked 0; attention_biases N(0, 1) (O(1) relative-position
+    structure, where torch's zero init would hide the bias indexing)."""
+    from mobile_sam.modeling.tiny_vit_sam import state_dict_shapes
+    gen = torch.Generator().manual_seed(seed)
+    out: Dict[str, torch.Tensor] = {}
+    for k, shp in sorted(state_dict_shapes(num_classes).items()):
+        leaf = k.rsplit(".", 1)[-1]
+        if leaf == "num_batches_tracked":
+            out[k] = torch.tensor(0, dtype=torch.long)
+        elif ".bn." in k and leaf == "weight":
+            out[k] = 0.5 + torch.rand(shp, generator=gen)
+        elif ".bn." in k and leaf in ("bias", "running_mean"):
+            out[k] = (torch.rand(shp, generator=gen) * 2 - 1) * 0.1
+        elif leaf == "running_var":
+            out[k] = 0.5 + 1.5 * torch.rand(shp, generator=gen)
+        elif leaf == "attention_biases":
+            out[k] = torch.randn(shp, generator=gen)
+        elif ".norm." in k:   # a non-zero LayerNorm bias makes the padded window tokens (LN(0) = bias) matter
+            out[k] = (1.0 if leaf == "weight" else 0.0) + (torch.rand(shp, generator=gen) * 2 - 1) * 0.3
+        else:
+            out[k] = _init_like_torch(k, shp, gen).float().contiguous()
+    return out
+
+
 def condition_pips(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     """x0.1 on the delta head makes random-weight PIPS contractive (SURVEY §0.4)."""
     sd = dict(sd)

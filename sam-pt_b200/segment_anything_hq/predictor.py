@@ -9,6 +9,17 @@ from segment_anything.predictor import SamPredictor as _Base
 
 
 class SamPredictor(_Base):
+    def __init__(self, sam_model) -> None:
+        # sam-hq's predictor unpacks (features, interm_embeddings) from the encoder and runs MaskDecoderHQ.  A plain SAM or
+        # MobileSAM model (sam_pt.yaml's default predictor with `model/sam@...=sam_mobile_vit_tiny`) would only fail on the
+        # first frame, so it is refused here.
+        if "hf_token.weight" not in sam_model.mask_decoder.state_dict():
+            raise ValueError(
+                f"segment_anything_hq.predictor.SamPredictor needs an HQ-SAM model (MaskDecoderHQ); "
+                f"{type(sam_model).__name__} has a {type(sam_model.mask_decoder).__name__}. For SAM or MobileSAM select the "
+                "plain predictor with model.sam_predictor._target_=segment_anything.predictor.SamPredictor")
+        super().__init__(sam_model)
+
     def _uses_interm(self) -> bool:
         return True
 
