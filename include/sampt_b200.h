@@ -312,6 +312,47 @@ int sampt_cotracker_window(sampt_ctx* ctx, const float* fmaps, const float* l1, 
                            const float* time_emb, int N, int iters, int time_depth, int space_depth, float* vis_out,
                            void* stream);
 
+/* ---- PIPS++ point tracker (csrc/pips_plus_plus.cu; sam_pt/point_tracker/pips_plus_plus/, weights "ppp.*") ---------------- */
+/* BasicEncoder at stride 8 over planar frames (T,3,H,W), uint8 (is_f32 = 0) or float32 holding 0..255 -> (T,H/8,W/8,128)
+ * channels-last; PipsPlusPlus.forward's `self.fnet(2*(rgbs/255)-1)` (pips_plus_plus.py:444-453), once per frame.  The pyramid
+ * is sampt_pips_pyramid's. */
+int sampt_pips_plus_plus_fnet(sampt_ctx* ctx, const void* frames, int is_f32, int T, int H, int W, float* fmaps, void* stream);
+/* PipsPlusPlus.forward on one window of S >= 2 frames (pips_plus_plus.py:436-546, inference): the pyramid (l0..l3) holds exactly
+ * the S frames; trajs_e0 (S,N,2) px; feat_init (3,S,N,128) = (feats1, feats2, feats4) or NULL -> coords_out (iters+1,S,N,2) px
+ * = coord_predictions1 (per iteration before frame 0 is re-locked, then the final locked coords), feats_out (3,S,N,128) = the
+ * returned `feats`.  The coarsest level must have at least 2 rows and columns: (H8 >> 3) >= 2 and (W8 >> 3) >= 2. */
+int sampt_pips_plus_plus_window(sampt_ctx* ctx, const float* l0, const float* l1, const float* l2, const float* l3, int H8, int W8,
+                                const float* trajs_e0, const float* feat_init, int N, int S, int stride, int iters,
+                                float* coords_out, float* feats_out, void* stream);
+/* PipsPlusPlusPointTracker._forward (pips_plus_plus/tracker.py:25-65) for one query group and one direction: window slot s of the
+ * pass reads pyramid frame t0 + dir*s (dir = -1: the time-reversed pass); Tdir frames; windows of max_len frames overlapping by
+ * one, the last one shifted back to end at Tdir, feat_init carried over.  query (N,2) px -> traj (Tdir,N,2) px in pass order. */
+int sampt_pips_plus_plus_track(sampt_ctx* ctx, const float* l0, const float* l1, const float* l2, const float* l3, int H8, int W8,
+                               int t0, int dir, int Tdir, const float* query, int N, int max_len, int stride, int iters, float* traj,
+                               void* stream);
+/* PipsPlusPlusPointTracker.forward's image_size resize (tracker.py:72-77): F.interpolate(rgbs/255, (Ho,Wo), bilinear,
+ * align_corners=False) * 255 over `planes` planar (H,W) frames, uint8 (is_f32 = 0) or float32 -> float32 (planes,Ho,Wo). */
+int sampt_pips_plus_plus_resize(sampt_ctx* ctx, const void* in, int is_f32, int planes, int H, int W, int Ho, int Wo, float* out,
+                                void* stream);
+/* Unit-test entries, through the launchers of sampt_pips_plus_plus_window with the registered "ppp.*" weights.
+ * row: the DeltaBlock input rows of one iteration; coords (S,N,2) feature-map px; feats (3,S,N,128) IN/OUT; mode 0 = targets as
+ * given, 1 = all three sampled at slot 0 (iteration 0), 2 = feats2 / feats4 resampled (iterations >= 1) -> row (N*S,718) fp32
+ * and A (N*S, 2*2176) fp16 hi|lo, the temporal im2col operand of first_block_conv. */
+int sampt_test_pips_plus_plus_row(sampt_ctx* ctx, const float* l0, const float* l1, const float* l2, const float* l3, int H8, int W8,
+                                  const float* coords, float* feats, int N, int S, int mode, float* row, void* A, void* stream);
+/* tconv: DeltaBlock Conv1dPad(k=3) `name` ("first_block_conv", "basicblock_list.<i>.conv1|conv2") on x (N*S,Cin) after pre = 0
+ * (none), 1 (ReLU) or 2 (ReLU(InstanceNorm1d)) -> out (N*S,Cout). */
+int sampt_test_pips_plus_plus_tconv(sampt_ctx* ctx, const char* name, const float* x, int N, int S, int Cin, int Cout, int pre,
+                                    float* out, void* stream);
+/* inorm: InstanceNorm1d over time, x (N*S,C) -> stats (N,C,2) = (mean, 1/sqrt(var + 1e-5)). */
+int sampt_test_pips_plus_plus_inorm(sampt_ctx* ctx, const float* x, int N, int S, int C, float* stats, void* stream);
+/* residual: block 0..7 = ResidualBlock1d on x (N*S,Cin) -> out (N*S,Cout) (block 0 applies DeltaBlock's first ReLU);
+ * block -1 = the whole DeltaBlock from the fp32 rows x (N*S,718) -> delta (N*S,2). */
+int sampt_test_pips_plus_plus_residual(sampt_ctx* ctx, int block, const float* x, int N, int S, float* out, void* stream);
+/* update: coords (S,N,2) += delta (N*S,2), then frame 0 <- lock (N,2); pre (S,N,2) or NULL = the pre-lock coords * stride. */
+int sampt_test_pips_plus_plus_update(sampt_ctx* ctx, float* coords, const float* lock, const float* delta, int N, int S, int stride,
+                                     float* pre, void* stream);
+
 /* ---- SURVEY §8(f) rows: the callers / data formats either side of the hot path ------------------------------------------- */
 /* Query points from masks (sam_pt/utils/query_points.py:64-104 -> sklearn_extra.cluster.KMedoids(n_clusters=k).fit(px)
  * .cluster_centers_, un-vendored scikit-learn-extra; defaults metric="euclidean", method="alternate", init="heuristic").

@@ -53,6 +53,11 @@ int pips_update(Ctx* c, cudaStream_t st, const PipsWin& w, const float* delta, c
                 const float* up_w, const float* up_b);
 int pips_link(Ctx* c, cudaStream_t st, const PipsWin& w, const float* vis_w, const float* vis_b, float thr0, int T);
 
+// ---- split-precision GEMM with a power-of-two weight scale (tinyvit.cu): Y[M, N] = act(A W^T 2^-s + bias) (+ resid), A and W
+// hi|lo with 2*Kp halves per row, W registered under `wname` and its accumulator scale 2^-s under `wname + "s"`
+int tv_gemm(Ctx* c, cudaStream_t st, const __half* A, const std::string& wname, int M, int N, int Kp, const float* bias, int act,
+            float* out32, const float* resid);
+
 }  // namespace sampt
 
 namespace sampt {

@@ -161,7 +161,10 @@ using namespace sampt;
 
 static int fnet_frames(Ctx* c, cudaStream_t st, const char* prefix, const void* frames, int is_f32, int T, int H, int W, int stride,
                        float* fmaps) {
-  SAMPT_CHECK(stride == 4, "fnet: only stride 4 (configs/model/point_tracker/pips.yaml:3, cotracker_stride_4_wind_8) is built, got %d", stride);
+  // stride 4: PIPS (configs/model/point_tracker/pips.yaml:3) and CoTracker (cotracker_stride_4_wind_8); stride 8: PIPS++ only
+  // (PipsPlusPlus(stride=8), weights "ppp.fnet.*")
+  SAMPT_CHECK(stride == 4 || (stride == 8 && std::string(prefix) == "ppp."),
+              "fnet: stride %d is not built for the '%s' encoder (4 for PIPS and CoTracker, 8 for PIPS++)", stride, prefix);
   c->fnet_prefix = prefix;
   const int Ho = H / stride, Wo = W / stride;
   // chunk frames so the fp32 half-res activations fit the workspace (6 buffers of n*H2*W2*64 floats + concat)
@@ -194,6 +197,13 @@ extern "C" int sampt_pips_fnet(sampt_ctx* ctx, const uint8_t* frames_u8, int T, 
 // 2*(x/255)-1 inside conv1 like upstream CoTracker.forward.
 extern "C" int sampt_cotracker_fnet(sampt_ctx* ctx, const float* frames_f32, int T, int H, int W, float* fmaps, void* stream) {
   return fnet_frames(reinterpret_cast<Ctx*>(ctx), reinterpret_cast<cudaStream_t>(stream), "cot.", frames_f32, 1, T, H, W, 4, fmaps);
+}
+
+// PIPS++'s BasicEncoder (same architecture, own weights under "ppp.fnet.*") at stride 8 over planar frames: uint8, or float32
+// holding 0..255 (the tracker's image_size resize); replaces PipsPlusPlus.forward's `self.fnet(2*(rgbs/255)-1)`, once per frame.
+extern "C" int sampt_pips_plus_plus_fnet(sampt_ctx* ctx, const void* frames, int is_f32, int T, int H, int W, float* fmaps,
+                                         void* stream) {
+  return fnet_frames(reinterpret_cast<Ctx*>(ctx), reinterpret_cast<cudaStream_t>(stream), "ppp.", frames, is_f32, T, H, W, 8, fmaps);
 }
 
 extern "C" int sampt_pips_pyramid(sampt_ctx* ctx, const float* fmaps, int T, int H4, int W4, float* l1, float* l2,

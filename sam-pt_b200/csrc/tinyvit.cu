@@ -317,8 +317,6 @@ int tv_window_attn(Ctx* c, cudaStream_t st, const float* qkv, const float* ab, _
 // ---------------------------------------------------------------------------------------------------------------------
 // Host side
 // ---------------------------------------------------------------------------------------------------------------------
-namespace {
-
 const std::string TV_PREFIX = "sam.tinyvit.";
 
 // three fp16 passes A_hi.B_hi + A_lo.B_hi + A_hi.B_lo over operands of 2*Kp halves per row
@@ -343,6 +341,8 @@ int tv_gemm(Ctx* c, cudaStream_t st, const __half* A, const std::string& wname, 
   ep.out32 = out32; ep.resid = resid; ep.bias = bias; ep.act = act; ep.ldc = N; ep.acc_scale = ws;
   return gemm_tc(c, st, A, 2 * Kp, w, 2 * Kp, M, N, Kp, seg3(Kp), ep);
 }
+
+namespace {
 
 struct TvBufs {
   float *X, *X2, *F, *QKV;

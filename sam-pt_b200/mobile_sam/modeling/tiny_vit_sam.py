@@ -15,7 +15,6 @@ Kernel-native layouts registered under "sam.tinyvit." (include/sampt_b200.h):
 """
 from __future__ import annotations
 
-import math
 from ctypes import c_float, c_int, c_size_t, byref
 from typing import Dict, List, Sequence, Tuple
 
@@ -23,6 +22,7 @@ import torch
 from torch import nn
 
 from sampt_b200 import native
+from sampt_b200.gemm_weights import split_scaled as _split
 from sampt_b200.param_tree import build_param_tree
 
 EMBED_DIMS = (64, 128, 160, 320)
@@ -107,21 +107,6 @@ def fold_conv_bn(sd: Dict[str, torch.Tensor], p: str) -> Tuple[torch.Tensor, tor
     rm, rv = sd[p + ".bn.running_mean"].double(), sd[p + ".bn.running_var"].double()
     scale = g / torch.sqrt(rv + BN_EPS)
     return w * scale.view(-1, 1, 1, 1), b - rm * scale
-
-
-def _split(wm: torch.Tensor, kp: int) -> Tuple[torch.Tensor, torch.Tensor]:
-    """[N, K] float64 -> ([N, 2*kp] fp16 hi | lo of w 2^s with zero columns K..kp in both halves, [2^-s] fp32).
-
-    The power of two 2^s puts max |w| 2^s in [2^14, 2^15): unscaled, the lo halves of weights of size ~1/sqrt(K) fall below
-    fp16's normal range (6.1e-5), where their absolute precision of 2^-24 costs ~2^-19 of every product.  Scaled, lo keeps
-    11 bits and the product error is the 2^-22 of the split itself.  gemm_tc multiplies the accumulator by 2^-s (exact)."""
-    w = torch.zeros((wm.shape[0], kp), dtype=torch.float32)
-    w[:, :wm.shape[1]] = wm.float()
-    amax = float(w.abs().max())
-    s = 15 - (math.frexp(amax)[1] if amax > 0 else 0)
-    w = w * (2.0 ** s)
-    hi = w.half()
-    return torch.cat([hi, (w - hi.float()).half()], dim=1).contiguous(), torch.tensor([2.0 ** -s], dtype=torch.float32)
 
 
 def native_weights(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:

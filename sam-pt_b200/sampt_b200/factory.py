@@ -89,7 +89,7 @@ def _build_tiny_sam(sam_state_dict, hq: bool):
 
 def build_sam_pt(vit: str, sam_state_dict, pips_ckpt_dir: str, positive_points_per_mask: int, negative_points_per_mask: int = 0,
                  iterative_refinement_iterations: int = 12, sam_iou_threshold: float = 0.7, device="cuda", hq: bool = False,
-                 cotracker_state_dict=None, cotracker_interp_shape=(384, 512)):
+                 cotracker_state_dict=None, cotracker_interp_shape=(384, 512), pips_plus_plus_state_dict=None):
     """configs/model/sam_pt.yaml with `model/point_tracker=pips`, `model/sam@...=sam_vit_*` and the demo-style overrides
     positive_points_per_mask=P negative_points_per_mask=0 (demo/demo.py:107-110)."""
     from sam_pt.modeling.sam_pt import SamPt
@@ -100,7 +100,12 @@ def build_sam_pt(vit: str, sam_state_dict, pips_ckpt_dir: str, positive_points_p
         from segment_anything.predictor import SamPredictor
 
     sam = build_sam(vit, sam_state_dict, hq=hq)
-    if cotracker_state_dict is not None:
+    if pips_plus_plus_state_dict is not None:
+        # configs/model/point_tracker/pips_plus_plus.yaml
+        from sam_pt.point_tracker.pips_plus_plus import PipsPlusPlusPointTracker
+        tracker = PipsPlusPlusPointTracker(checkpoint_path=None, stride=8, max_sequence_length=128, iters=16, image_size=None)
+        tracker.model.load_state_dict(pips_plus_plus_state_dict)
+    elif cotracker_state_dict is not None:
         # configs/model/point_tracker/cotracker.yaml (the reference's default tracker group)
         from sam_pt.point_tracker.cotracker import CoTrackerPointTracker
         tracker = CoTrackerPointTracker(checkpoint_path=None, interp_shape=list(cotracker_interp_shape), visibility_threshold=0.7, support_grid_size=2,

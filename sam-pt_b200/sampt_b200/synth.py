@@ -166,6 +166,22 @@ def condition_pips(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     return sd
 
 
+def make_pips_plus_plus_state_dict(seed: int = 8201) -> Dict[str, torch.Tensor]:
+    from sam_pt.point_tracker.pips_plus_plus.pips_plus_plus import state_dict_shapes
+    return condition_pips_plus_plus(make_state_dict(state_dict_shapes(), seed))
+
+
+def condition_pips_plus_plus(sd: Dict[str, torch.Tensor], scale: float = 0.03) -> Dict[str, torch.Tensor]:
+    """Untrained, the DeltaBlock moves points by ~6 px per iteration and the 16-iteration chain wanders off (73 px after 16
+    iterations at 128x160; float32 and float64 runs of it end 14 px apart).  x0.03 on `delta_block.dense`, as x0.1 on PIPS's
+    delta head, makes it contractive: 2.5 px of motion after 16 iterations, float32 vs float64 5.6e-5 px (x0.1 still leaves
+    4.1e-4 px)."""
+    sd = dict(sd)
+    sd["delta_block.dense.weight"] = sd["delta_block.dense.weight"] * scale
+    sd["delta_block.dense.bias"] = sd["delta_block.dense.bias"] * scale
+    return sd
+
+
 def condition_sam(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     """Make random-weight SAM produce non-degenerate, well-separated mask logits: give the mask-0 hyper-network
     a strong constant component so `logit = hyper . upscaled` has O(1) structure instead of ~0 noise (SURVEY §8d)."""
