@@ -81,7 +81,7 @@ int sampt_pips_corr_lookup(sampt_ctx* ctx, const float* fmaps, const float* l1, 
                            int H4, int W4, const float* ffeats, const float* coords, int N, float* fcorr, void* stream);
 
 /* ---- generic fp32 linear (unit tests; torch.nn.functional.linear semantics) ----------------------------------- */
-/* Y[M,N] = act(X[M,K] W[N,K]^T + bias) (+ residual); act 0 none / 1 GELU(erf) / 2 ReLU; K,ldx,ldw multiples of 4 */
+/* Y[M,N] = act(X[M,K] W[N,K]^T + bias) (+ residual); act 0 none / 1 GELU(erf) / 2 ReLU / 3 GELU(tanh); K,ldx,ldw multiples of 4 */
 int sampt_linear_f32(sampt_ctx* ctx, const float* X, int ldx, const float* W, int ldw, const float* bias,
                      const float* residual, int ldr, float* Y, int ldy, int M, int N, int K, int act, void* stream);
 
@@ -118,8 +118,9 @@ int sampt_attention_f16(sampt_ctx* ctx, const void* Qx, const void* Kx, const vo
                         int HD, int NT, int nheads, void* out, int ld_out, int split_off, void* stream);
 
 /* ---- unit-test entries, not used by the Python package -------------------------------------------------------------- */
-/* Eleven entries: the ViT's tensor-core GEMM and attention block (below), four stages of the SAM prompt encoder / mask
- * decoder (attention cores, prompt encoder, upscaling tail, postprocess + refinement control), then five of the PIPS tracker. */
+/* Twenty-six entries in all.  Here: the ViT's tensor-core GEMM and attention block, four stages of the SAM prompt encoder / mask
+ * decoder (attention cores, prompt encoder, upscaling tail, postprocess + refinement control), five of the PIPS tracker and five
+ * of the CoTracker window.  The five TinyViT and five PIPS++ entries are declared in their own sections. */
 /* The ViT's tensor-core GEMM (csrc/gemm_tc.cu, csrc/tc_api.cuh) with every option the pipelines use:
  * C = epilogue(sum over segments i < nseg of A[:, a_off[i] : +K] . B[:, b_off[i] : +K]^T)   (offsets in fp16 units; f8[i] != 0:
  * the segment holds K e4m3 bytes).  a_off_host / b_off_host / f8_host are HOST int[nseg].  Epilogue, in this order: times
@@ -197,6 +198,27 @@ int sampt_test_pips_window_op(sampt_ctx* ctx, int op, int N, int S, int T, int s
                               const uint8_t* active_host, const float* fmaps, int H4, int W4, float* coords, float* ffeats,
                               float* feat_init, float* traj, float* vis, int* cur, float* x, float* xln, int layer,
                               const float* delta, float thr0, void* stream);
+/* Five stages of the CoTracker window (csrc/cotracker.cu) through the launchers of sampt_cotracker_window, with the registered
+ * "cot.*" weights.  S = 8 slots, M = 8 N token rows (row = n*8 + s).
+ * input: pos (N,456) = the sincos position table sampled at slot 0's coordinate, then xin (N*8,456) = the transformer input rows;
+ *   pyramid levels (frames,H_l,W_l,128), slots_host HOST int[8] = the frame feeding each slot, coords (N,8,2) feature px,
+ *   ffeats (N,8,128), track_mask / vis_init (N,8), time_emb (8,456).
+ * ln: op 0 = LayerNorm (no affine, eps 1e-6) of x [M,384] -> y32 [M,384]; op 1 = the same into y16 [M,768] fp16 hi | lo;
+ *   op 2 = split x [M,K] -> y16 [M,2K] fp16 hi | lo (K a multiple of 4).
+ * attn: the attention core on qkv [M,1152] -> out [M,384] for G groups of L tokens, token row = g*gstride + l*lstride; qsplit
+ *   (1..8) CTAs share a group's queries, 0 = the window's choice.  Groups that do not fit shared memory are an error.
+ * block: one UpdateFormer block (kind 0 = time_blocks.<blk>, 1 = space_blocks.<blk>) on x (N*8,384) in place; tc = 1 runs its four
+ *   GEMMs on tensor cores (three fp16 hi | lo passes, needs the ".w16" weights), tc = 0 on the fp32 CUDA cores.
+ * update: ffeats (N,8,128) += GELU(Linear(GroupNorm(delta[:, 2:]))), coords (N,8,2) += delta[:, :2] from delta (N*8,130), then
+ *   vis_out (N,8) = the visibility head's logits. */
+int sampt_test_cotracker_input(sampt_ctx* ctx, const float* fmaps, const float* l1, const float* l2, const float* l3, int H4, int W4,
+                               const int* slots_host, const float* coords, const float* ffeats, const float* track_mask,
+                               const float* vis_init, const float* time_emb, int N, float* pos, float* xin, void* stream);
+int sampt_test_cotracker_ln(sampt_ctx* ctx, int op, const float* x, int M, int K, float* y32, void* y16, void* stream);
+int sampt_test_cotracker_attn(sampt_ctx* ctx, const float* qkv, float* out, int G, int L, int gstride, int lstride, int qsplit,
+                              void* stream);
+int sampt_test_cotracker_block(sampt_ctx* ctx, int kind, int blk, int tc, float* x, int N, void* stream);
+int sampt_test_cotracker_update(sampt_ctx* ctx, const float* delta, float* coords, float* ffeats, int N, float* vis_out, void* stream);
 
 /* ---- SAM image encoder ------------------------------------------------------------------------------------------ */
 /* ResizeLongestSide.apply_image (PIL bilinear, bit-exact): planar uint8 (B,3,H,W) -> (B,3,Ho,Wo); coefficient tables

@@ -31,12 +31,12 @@ IN_DIM = 456  # 130 (flow emb) + 196 (corr) + 128 (feat) + 2 (track mask, vis)
 
 # ----------------------------------------------------------------------------- embeddings (upstream models/core/embeddings.py)
 def get_2d_embedding(xy, C=64):
-    """(B,N,2) -> (B,N,2C+2) = [xy | sincos(x) | sincos(y)]  ([unverified]: coordinate columns first)."""
-    div = (torch.arange(0, C, 2, dtype=torch.float32) * (1000.0 / C)).reshape(1, 1, C // 2)
+    """(B,N,2) -> (B,N,2C+2) = [xy | sincos(x) | sincos(y)]  ([unverified]: coordinate columns first), in xy's dtype."""
+    div = (torch.arange(0, C, 2, dtype=xy.dtype, device=xy.device) * (1000.0 / C)).reshape(1, 1, C // 2)
     out = [xy]
     for d in range(2):
         v = xy[:, :, d:d + 1]
-        pe = torch.zeros(xy.shape[0], xy.shape[1], C)
+        pe = torch.zeros(xy.shape[0], xy.shape[1], C, dtype=xy.dtype, device=xy.device)
         pe[:, :, 0::2] = torch.sin(v * div)
         pe[:, :, 1::2] = torch.cos(v * div)
         out.append(pe)
@@ -61,14 +61,15 @@ def get_2d_sincos_pos_embed(embed_dim: int, grid_hw: Tuple[int, int]) -> np.ndar
 
 
 def sample_pos_embed(grid_hw, embed_dim, coords0):
-    """bilinear sample of the 2-D table at the window's first-frame coords: (B,N,2) -> (B,N,D)."""
-    tab = torch.from_numpy(get_2d_sincos_pos_embed(embed_dim, grid_hw)).float().reshape(1, grid_hw[0], grid_hw[1], embed_dim)
+    """bilinear sample of the 2-D table (float64, rounded to coords0's dtype) at the window's first-frame coords: (B,N,2) -> (B,N,D)."""
+    tab = torch.from_numpy(get_2d_sincos_pos_embed(embed_dim, grid_hw)).to(dtype=coords0.dtype, device=coords0.device)
+    tab = tab.reshape(1, grid_hw[0], grid_hw[1], embed_dim)
     s = pips_ref.bilinear_sample2d(tab.permute(0, 3, 1, 2), coords0[:, :, 0], coords0[:, :, 1])
     return s.permute(0, 2, 1)
 
 
-def time_embed(embed_dim: int, S: int):
-    return torch.from_numpy(_sincos_1d(embed_dim, np.linspace(0, S - 1, S))).float()  # (S, D)
+def time_embed(embed_dim: int, S: int, dtype=torch.float32, device=None):
+    return torch.from_numpy(_sincos_1d(embed_dim, np.linspace(0, S - 1, S))).to(dtype=dtype, device=device)  # (S, D)
 
 
 # ----------------------------------------------------------------------------- UpdateFormer
@@ -114,7 +115,7 @@ def forward_iteration(sd: SD, fmaps, coords_init, feat_init, vis_init, track_mas
     ffeats = feat_init.clone()
     pos = sample_pos_embed((H4, W4), IN_DIM, coords[:, 0])           # (1,N,456)
     pos = pos.reshape(B * N, 1, IN_DIM)
-    tim = time_embed(IN_DIM, S)[None]                                # (1,S,456)
+    tim = time_embed(IN_DIM, S, coords.dtype, coords.device)[None]   # (1,S,456)
     if track_mask.shape[1] < S:
         track_mask = torch.cat([track_mask, torch.zeros_like(track_mask[:, :1]).repeat(1, S - track_mask.shape[1], 1, 1)], dim=1)
     preds = []
@@ -124,7 +125,7 @@ def forward_iteration(sd: SD, fmaps, coords_init, feat_init, vis_init, track_mas
         flows_ = (coords - coords[:, 0:1]).permute(0, 2, 1, 3).reshape(B * N, S, 2)
         flows_cat = get_2d_embedding(flows_, 64)                      # (BN,S,130)
         ffeats_ = ffeats.permute(0, 2, 1, 3).reshape(B * N, S, LATENT)
-        concat = torch.cat([track_mask.float(), vis_init], dim=3).permute(0, 2, 1, 3).reshape(B * N, S, 2)
+        concat = torch.cat([track_mask.to(vis_init.dtype), vis_init], dim=3).permute(0, 2, 1, 3).reshape(B * N, S, 2)
         x = torch.cat([flows_cat, fcorrs_, ffeats_, concat], dim=2) + pos + tim
         delta = update_former(sd, x.reshape(B, N, S, IN_DIM)).reshape(B * N, S, LATENT + 2)
         dcoords, dfeats = delta[:, :, :2], delta[:, :, 2:].reshape(B * N * S, LATENT)
@@ -141,7 +142,8 @@ def forward_iteration(sd: SD, fmaps, coords_init, feat_init, vis_init, track_mas
 # ----------------------------------------------------------------------------- CoTracker.forward (sliding windows, step S/2)
 @torch.no_grad()
 def cotracker_forward(sd: SD, rgbs, queries, iters=6, stride=4, S=8, fmaps_all: Optional[torch.Tensor] = None):
-    """rgbs (1,T,3,H,W) float 0..255 at the interp resolution; queries (1,N,3)=(t,x,y) -> traj (1,T,N,2) px, vis (1,T,N) sigmoid.
+    """rgbs (1,T,3,H,W) float 0..255 at the interp resolution; queries (1,N,3)=(t,x,y) -> traj (1,T,N,2) px, vis (1,T,N) sigmoid,
+    in the dtype and on the device of `queries`.
     `fmaps_all` (T,128,H/4,W/4): encoder output computed once per frame (results-neutral; upstream re-encodes S/2 frames per window)."""
     B, T, C, H, W = rgbs.shape
     N = queries.shape[1]
@@ -154,11 +156,12 @@ def cotracker_forward(sd: SD, rgbs, queries, iters=6, stride=4, S=8, fmaps_all: 
     if fmaps_all is None:
         x = 2 * (rgbs[0] / 255.0) - 1.0
         fmaps_all = torch.cat([pips_ref.fnet(sd, x[i:i + 1], stride) for i in range(T)], dim=0)
-    traj_e = torch.zeros((B, T, N, 2))
-    vis_e = torch.zeros((B, T, N))
-    ind_array = torch.arange(T).repeat(B, 1)
+    dt, dev = queries.dtype, queries.device
+    traj_e = torch.zeros((B, T, N, 2), dtype=dt, device=dev)
+    vis_e = torch.zeros((B, T, N), dtype=dt, device=dev)
+    ind_array = torch.arange(T, device=dev).repeat(B, 1)
     track_mask = (ind_array[:, :, None] >= first[:, None, :]).unsqueeze(-1)
-    vis_init = torch.ones((B, S, N, 1)) * 10
+    vis_init = torch.ones((B, S, N, 1), dtype=dt, device=dev) * 10
     track_mask_ = track_mask[:, :, sort_inds].clone()
     coords_init_ = coords_init[:, :, sort_inds].clone()
     vis_init_ = vis_init[:, :, sort_inds].clone()

@@ -360,43 +360,118 @@ static int cot_tcg(Ctx* c, cudaStream_t st, const __half* X16, const __half* W16
   return gemm_tc(c, st, X16, 2 * K, W16, 2 * K, M, N, K, seg, ep);
 }
 
-// AttnBlock: x += proj(attn(LN(x))) ; x += fc2(gelu_tanh(fc1(LN(x))))    (groups: G x L tokens)
-static int attn_block(Ctx* c, cudaStream_t st, const CotBlockW& w, CotBufs& b, int M, int G, int L, int gstride, int lstride) {
-  const bool tc = b.h16 != nullptr && w.qkv_w16 != nullptr;
-  if (tc) {
-    ln384_split_kernel<<<cdiv(M, 8), 256, 0, st>>>(b.x, b.h16, M);
-    c->launches++;
-    SAMPT_TRY(cot_tcg(c, st, b.h16, w.qkv_w16, w.qkv_b, nullptr, b.qkv, nullptr, 0, M, 3 * CT_HID, CT_HID));
-  } else {
-    ln384_kernel<<<cdiv(M, 8), 256, 0, st>>>(b.x, b.h, M);
-    c->launches++;
-    SAMPT_TRY(sgemm_nt(c, st, b.h, CT_HID, w.qkv_w, CT_HID, w.qkv_b, nullptr, 0, b.qkv, 3 * CT_HID, M, 3 * CT_HID, CT_HID, 0));
-  }
+// LayerNorm of M rows: fp32 into y32, or the fp16 hi | lo operand of the tensor-core path into y16 (exactly one is non-null)
+static int cot_ln(Ctx* c, cudaStream_t st, const float* x, float* y32, __half* y16, int M) {
+  if (y16) ln384_split_kernel<<<cdiv(M, 8), 256, 0, st>>>(x, y16, M);
+  else ln384_kernel<<<cdiv(M, 8), 256, 0, st>>>(x, y32, M);
+  c->launches++;
+  SAMPT_LAUNCH_CHECK();
+  return 0;
+}
+
+// x [M, K] fp32 -> fp16 hi | lo [M, 2K]
+static int cot_split(Ctx* c, cudaStream_t st, const float* x, __half* out, int M, int K) {
+  const long long n4 = (long long)M * K / 4;
+  cot_split_kernel<<<cdiv(n4, 256), 256, 0, st>>>(x, out, n4, K);
+  c->launches++;
+  SAMPT_LAUNCH_CHECK();
+  return 0;
+}
+
+// attention core over G groups of L tokens.  qsplit CTAs share a group's queries; qsplit <= 0 picks the count the window uses
+// (double it while the grid is under two waves and every chunk keeps >= 8 queries).
+static int cot_attn(Ctx* c, cudaStream_t st, const float* qkv, float* out, int G, int L, int gstride, int lstride, int qsplit) {
   size_t smem = ((size_t)L * 49 * 2 + (size_t)8 * L) * sizeof(float);
   SAMPT_CHECK(smem <= 200 * 1024, "cot_attn: %d tokens per group do not fit shared memory", L);
   SAMPT_TRY(ensure_func_smem(c, "cot_attn_kernel", cot_attn_kernel, 200 * 1024));
-  int qsplit = 1;
-  while (qsplit < 8 && G * CT_HEADS * qsplit < 2 * c->num_sms && L / (2 * qsplit) >= 8) qsplit *= 2;
-  cot_attn_kernel<<<dim3(G, CT_HEADS, qsplit), 256, smem, st>>>(b.qkv, b.att, L, gstride, lstride);
+  if (qsplit <= 0) {
+    qsplit = 1;
+    while (qsplit < 8 && G * CT_HEADS * qsplit < 2 * c->num_sms && L / (2 * qsplit) >= 8) qsplit *= 2;
+  }
+  cot_attn_kernel<<<dim3(G, CT_HEADS, qsplit), 256, smem, st>>>(qkv, out, L, gstride, lstride);
   c->launches++;
   SAMPT_LAUNCH_CHECK();
+  return 0;
+}
+
+// AttnBlock: x += proj(attn(LN(x))) ; x += fc2(gelu_tanh(fc1(LN(x))))    (groups: G x L tokens)
+// tc: the four GEMMs on tensor cores (three fp16 hi | lo passes; needs the ".w16" weights and b.h16 / att16 / mlp16), else fp32 sgemm
+static int attn_block(Ctx* c, cudaStream_t st, const CotBlockW& w, CotBufs& b, bool tc, int M, int G, int L, int gstride, int lstride) {
   if (tc) {
-    const long long n4 = (long long)M * CT_HID / 4;
-    cot_split_kernel<<<cdiv(n4, 256), 256, 0, st>>>(b.att, b.att16, n4, CT_HID);
-    c->launches++;
+    SAMPT_CHECK(w.qkv_w16 != nullptr && b.h16 != nullptr, "cot attn_block: the tensor-core path needs the .w16 weights");
+    SAMPT_TRY(cot_ln(c, st, b.x, nullptr, b.h16, M));
+    SAMPT_TRY(cot_tcg(c, st, b.h16, w.qkv_w16, w.qkv_b, nullptr, b.qkv, nullptr, 0, M, 3 * CT_HID, CT_HID));
+  } else {
+    SAMPT_TRY(cot_ln(c, st, b.x, b.h, nullptr, M));
+    SAMPT_TRY(sgemm_nt(c, st, b.h, CT_HID, w.qkv_w, CT_HID, w.qkv_b, nullptr, 0, b.qkv, 3 * CT_HID, M, 3 * CT_HID, CT_HID, 0));
+  }
+  SAMPT_TRY(cot_attn(c, st, b.qkv, b.att, G, L, gstride, lstride, 0));
+  if (tc) {
+    SAMPT_TRY(cot_split(c, st, b.att, b.att16, M, CT_HID));
     SAMPT_TRY(cot_tcg(c, st, b.att16, w.proj_w16, w.proj_b, b.x, b.x, nullptr, 0, M, CT_HID, CT_HID));
-    ln384_split_kernel<<<cdiv(M, 8), 256, 0, st>>>(b.x, b.h16, M);
-    c->launches++;
+    SAMPT_TRY(cot_ln(c, st, b.x, nullptr, b.h16, M));
     SAMPT_TRY(cot_tcg(c, st, b.h16, w.fc1_w16, w.fc1_b, nullptr, nullptr, b.mlp16, 3, M, 4 * CT_HID, CT_HID));   // GELU(tanh), hi | lo out
     SAMPT_TRY(cot_tcg(c, st, b.mlp16, w.fc2_w16, w.fc2_b, b.x, b.x, nullptr, 0, M, CT_HID, 4 * CT_HID));
     return 0;
   }
   SAMPT_TRY(sgemm_nt(c, st, b.att, CT_HID, w.proj_w, CT_HID, w.proj_b, b.x, CT_HID, b.x, CT_HID, M, CT_HID, CT_HID, 0));
-  ln384_kernel<<<cdiv(M, 8), 256, 0, st>>>(b.x, b.h, M);
-  c->launches++;
+  SAMPT_TRY(cot_ln(c, st, b.x, b.h, nullptr, M));
   SAMPT_TRY(sgemm_nt(c, st, b.h, CT_HID, w.fc1_w, CT_HID, w.fc1_b, nullptr, 0, b.mlp, 4 * CT_HID, M, 4 * CT_HID, CT_HID, 3));
   SAMPT_TRY(sgemm_nt(c, st, b.mlp, 4 * CT_HID, w.fc2_w, 4 * CT_HID, w.fc2_b, b.x, CT_HID, b.x, CT_HID, M, CT_HID, 4 * CT_HID, 0));
   return 0;
+}
+
+// GroupNorm / ffeat updater / visibility head weights
+struct CotHeadW {
+  const float *gn_w, *gn_b, *up_w, *up_b, *vis_w, *vis_b;
+};
+
+static int load_head(Ctx* c, CotHeadW* h) {
+  SAMPT_TRY(get_f32(c, "cot.norm.weight", &h->gn_w)); SAMPT_TRY(get_f32(c, "cot.norm.bias", &h->gn_b));
+  SAMPT_TRY(get_f32(c, "cot.ffeat_updater.0.weight", &h->up_w)); SAMPT_TRY(get_f32(c, "cot.ffeat_updater.0.bias", &h->up_b));
+  SAMPT_TRY(get_f32(c, "cot.vis_predictor.0.weight", &h->vis_w)); SAMPT_TRY(get_f32(c, "cot.vis_predictor.0.bias", &h->vis_b));
+  return 0;
+}
+
+static int cot_pos(Ctx* c, cudaStream_t st, const PipsWin& w, float* pos) {
+  cot_pos_kernel<<<w.N, 256, 0, st>>>(w, pos);
+  c->launches++;
+  SAMPT_LAUNCH_CHECK();
+  return 0;
+}
+
+static int cot_input(Ctx* c, cudaStream_t st, const PipsWin& w, const float* track_mask, const float* vis_init, const float* time_emb,
+                     const float* pos, float* xin) {
+  cot_input_kernel<<<w.N * w.S, 256, 0, st>>>(w, track_mask, vis_init, time_emb, pos, xin);
+  c->launches++;
+  SAMPT_LAUNCH_CHECK();
+  return 0;
+}
+
+static int cot_update(Ctx* c, cudaStream_t st, const PipsWin& w, const float* delta, const CotHeadW& h) {
+  cot_update_kernel<<<w.N * w.S, 128, 0, st>>>(w, delta, h.gn_w, h.gn_b, h.up_w, h.up_b);
+  c->launches++;
+  SAMPT_LAUNCH_CHECK();
+  return 0;
+}
+
+static int cot_vis(Ctx* c, cudaStream_t st, const PipsWin& w, const CotHeadW& h, float* vis_out) {
+  cot_vis_kernel<<<cdiv(w.N * w.S, 128), 128, 0, st>>>(w, h.vis_w, h.vis_b, vis_out);
+  c->launches++;
+  SAMPT_LAUNCH_CHECK();
+  return 0;
+}
+
+static PipsWin cot_win(const float* fmaps, const float* l1, const float* l2, const float* l3, int H4, int W4, const int* fidx_dev,
+                       float* coords, float* ffeats, int N) {
+  PipsWin w{};
+  w.N = N; w.S = 8; w.stride = 4; w.T = 8;
+  w.pyr[0] = fmaps; w.pyr[1] = l1; w.pyr[2] = l2; w.pyr[3] = l3;
+  w.H[0] = H4; w.W[0] = W4;
+  for (int l = 1; l < 4; ++l) { w.H[l] = w.H[l - 1] / 2; w.W[l] = w.W[l - 1] / 2; }
+  w.coords = coords; w.ffeats = ffeats;
+  w.wp = fidx_dev;
+  return w;
 }
 
 }  // namespace sampt
@@ -421,19 +496,12 @@ extern "C" int sampt_cotracker_window(sampt_ctx* ctx, const float* fmaps, const 
   std::vector<CotBlockW> tb(time_depth), sb(space_depth);
   for (int i = 0; i < time_depth; ++i) SAMPT_TRY(load_block(c, p + "time_blocks." + std::to_string(i) + ".", &tb[i]));
   for (int i = 0; i < space_depth; ++i) SAMPT_TRY(load_block(c, p + "space_blocks." + std::to_string(i) + ".", &sb[i]));
-  const float *in_w, *in_b, *fh_w, *fh_b, *gn_w, *gn_b, *up_w, *up_b, *vis_w, *vis_b;
+  const float *in_w, *in_b, *fh_w, *fh_b;
   SAMPT_TRY(get_f32(c, p + "input_transform.weight", &in_w)); SAMPT_TRY(get_f32(c, p + "input_transform.bias", &in_b));
   SAMPT_TRY(get_f32(c, p + "flow_head.weight", &fh_w)); SAMPT_TRY(get_f32(c, p + "flow_head.bias", &fh_b));
-  SAMPT_TRY(get_f32(c, "cot.norm.weight", &gn_w)); SAMPT_TRY(get_f32(c, "cot.norm.bias", &gn_b));
-  SAMPT_TRY(get_f32(c, "cot.ffeat_updater.0.weight", &up_w)); SAMPT_TRY(get_f32(c, "cot.ffeat_updater.0.bias", &up_b));
-  SAMPT_TRY(get_f32(c, "cot.vis_predictor.0.weight", &vis_w)); SAMPT_TRY(get_f32(c, "cot.vis_predictor.0.bias", &vis_b));
-  PipsWin w{};
-  w.N = N; w.S = S; w.stride = 4; w.T = S;
-  w.pyr[0] = fmaps; w.pyr[1] = l1; w.pyr[2] = l2; w.pyr[3] = l3;
-  w.H[0] = H4; w.W[0] = W4;
-  for (int l = 1; l < 4; ++l) { w.H[l] = w.H[l - 1] / 2; w.W[l] = w.W[l - 1] / 2; }
-  w.coords = coords; w.ffeats = ffeats;
-  w.wp = fidx_dev;
+  CotHeadW hw;
+  SAMPT_TRY(load_head(c, &hw));
+  const PipsWin w = cot_win(fmaps, l1, l2, l3, H4, W4, fidx_dev, coords, ffeats, N);
   CotBufs b;
   float *xin, *delta, *pos;
   SAMPT_TRY(ws_get(c, &xin, (size_t)M * CT_IN, "cot xin"));
@@ -447,38 +515,32 @@ extern "C" int sampt_cotracker_window(sampt_ctx* ctx, const float* fmaps, const 
   // UpdateFormer GEMMs on tensor cores (three fp16 hi | lo passes) once the token count fills 128-row tiles; SAMPT_COT_TC=0 keeps fp32
   static const int cot_tc_on = [] { const char* e = std::getenv("SAMPT_COT_TC"); return (e != nullptr && e[0] == '0') ? 0 : 1; }();
   b.h16 = b.att16 = b.mlp16 = nullptr;
-  if (cot_tc_on && M >= 128 && tb[0].qkv_w16 != nullptr) {
+  // (each block then runs on tensor cores when its own ".w16" weights are registered)
+  const bool tc = cot_tc_on && M >= 128 && tb[0].qkv_w16 != nullptr;
+  if (tc) {
     SAMPT_TRY(ws_get(c, &b.h16, (size_t)M * 2 * CT_HID, "cot h16"));
     SAMPT_TRY(ws_get(c, &b.att16, (size_t)M * 2 * CT_HID, "cot att16"));
     SAMPT_TRY(ws_get(c, &b.mlp16, (size_t)M * 8 * CT_HID, "cot mlp16"));
   }
-  cot_pos_kernel<<<N, 256, 0, st>>>(w, pos);
-  c->launches++;
+  SAMPT_TRY(cot_pos(c, st, w, pos));
   for (int it = 0; it < iters; ++it) {
-    cot_input_kernel<<<M, 256, 0, st>>>(w, track_mask, vis_init, time_emb, pos, xin);
-    c->launches++;
-    SAMPT_LAUNCH_CHECK();
+    SAMPT_TRY(cot_input(c, st, w, track_mask, vis_init, time_emb, pos, xin));
     SAMPT_TRY(sgemm_nt(c, st, xin, CT_IN, in_w, CT_IN, in_b, nullptr, 0, b.x, CT_HID, M, CT_HID, CT_IN, 0));
     int j = 0;
     for (int i = 0; i < time_depth; ++i) {
       // time attention: N groups of S consecutive tokens (token row = n*S + s)
-      SAMPT_TRY(attn_block(c, st, tb[i], b, M, N, S, S, 1));
+      SAMPT_TRY(attn_block(c, st, tb[i], b, tc && tb[i].qkv_w16 != nullptr, M, N, S, S, 1));
       if (i % (time_depth / space_depth) == 0) {
         // space attention: S groups of N tokens (row = s + n*S)
-        SAMPT_TRY(attn_block(c, st, sb[j], b, M, S, N, 1, S));
+        SAMPT_TRY(attn_block(c, st, sb[j], b, tc && sb[j].qkv_w16 != nullptr, M, S, N, 1, S));
         ++j;
       }
     }
     // flow_head: 384 -> 130
     SAMPT_TRY(sgemm_nt(c, st, b.x, CT_HID, fh_w, CT_HID, fh_b, nullptr, 0, delta, 130, M, 130, CT_HID, 0));
-    cot_update_kernel<<<M, 128, 0, st>>>(w, delta, gn_w, gn_b, up_w, up_b);
-    c->launches++;
-    SAMPT_LAUNCH_CHECK();
+    SAMPT_TRY(cot_update(c, st, w, delta, hw));
   }
-  cot_vis_kernel<<<cdiv(M, 128), 128, 0, st>>>(w, vis_w, vis_b, vis_out);
-  c->launches++;
-  SAMPT_LAUNCH_CHECK();
-  return 0;
+  return cot_vis(c, st, w, hw, vis_out);
 }
 
 extern "C" int sampt_resize_bilinear_u8_f32(sampt_ctx* ctx, const uint8_t* in, int planes, int H, int W, int Ho, int Wo, float* out,
@@ -501,4 +563,86 @@ extern "C" int sampt_cotracker_sample_features(sampt_ctx* ctx, const float* fmap
   c->launches++;
   SAMPT_LAUNCH_CHECK();
   return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// unit-test entries (include/sampt_b200.h): each runs the launchers of sampt_cotracker_window on caller-owned buffers
+// ---------------------------------------------------------------------------------------------------------------------
+extern "C" int sampt_test_cotracker_input(sampt_ctx* ctx, const float* fmaps, const float* l1, const float* l2, const float* l3, int H4,
+                                          int W4, const int* slots_host, const float* coords, const float* ffeats, const float* track_mask,
+                                          const float* vis_init, const float* time_emb, int N, float* pos, float* xin, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(N >= 1 && slots_host != nullptr, "sampt_test_cotracker_input: N positive and 8 slot frames required");
+  c->ws_reset();
+  int fidx_h[10] = {0, 0};
+  for (int s = 0; s < 8; ++s) fidx_h[2 + s] = slots_host[s];
+  int* fidx_d;
+  SAMPT_TRY(ws_get(c, &fidx_d, 16, "cot test slots"));
+  SAMPT_CUDA(cudaMemcpyAsync(fidx_d, fidx_h, sizeof(fidx_h), cudaMemcpyHostToDevice, st));
+  SAMPT_CUDA(cudaStreamSynchronize(st));
+  const PipsWin w = cot_win(fmaps, l1, l2, l3, H4, W4, fidx_d, const_cast<float*>(coords), const_cast<float*>(ffeats), N);
+  SAMPT_TRY(cot_pos(c, st, w, pos));
+  return cot_input(c, st, w, track_mask, vis_init, time_emb, pos, xin);
+}
+
+extern "C" int sampt_test_cotracker_ln(sampt_ctx* ctx, int op, const float* x, int M, int K, float* y32, void* y16, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(M >= 1, "sampt_test_cotracker_ln: no rows");
+  switch (op) {
+    case 0:
+    case 1:
+      SAMPT_CHECK(K == CT_HID, "sampt_test_cotracker_ln: LayerNorm rows have %d channels", CT_HID);
+      return cot_ln(c, st, x, op == 0 ? y32 : nullptr, op == 1 ? static_cast<__half*>(y16) : nullptr, M);
+    case 2:
+      SAMPT_CHECK(K >= 4 && K % 4 == 0, "sampt_test_cotracker_ln: split needs K a positive multiple of 4");
+      return cot_split(c, st, x, static_cast<__half*>(y16), M, K);
+    default:
+      set_error("sampt_test_cotracker_ln: unknown op %d", op);
+      return -2;
+  }
+}
+
+extern "C" int sampt_test_cotracker_attn(sampt_ctx* ctx, const float* qkv, float* out, int G, int L, int gstride, int lstride, int qsplit,
+                                         void* stream) {
+  SAMPT_CHECK(G >= 1 && L >= 1 && qsplit <= 8, "sampt_test_cotracker_attn: G, L positive and qsplit <= 8 required");
+  return cot_attn(reinterpret_cast<Ctx*>(ctx), reinterpret_cast<cudaStream_t>(stream), qkv, out, G, L, gstride, lstride, qsplit);
+}
+
+extern "C" int sampt_test_cotracker_block(sampt_ctx* ctx, int kind, int blk, int tc, float* x, int N, void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK((kind == 0 || kind == 1) && N >= 1, "sampt_test_cotracker_block: kind 0 (time) or 1 (space), N positive");
+  c->ws_reset();
+  const int S = 8, M = N * S;
+  CotBlockW w;
+  SAMPT_TRY(load_block(c, std::string("cot.updateformer.") + (kind ? "space_blocks." : "time_blocks.") + std::to_string(blk) + ".", &w));
+  SAMPT_CHECK(!tc || w.qkv_w16 != nullptr, "sampt_test_cotracker_block: tc = 1 needs the .w16 weights");
+  CotBufs b;
+  b.x = x;
+  SAMPT_TRY(ws_get(c, &b.h, (size_t)M * CT_HID, "cot h"));
+  SAMPT_TRY(ws_get(c, &b.qkv, (size_t)M * 3 * CT_HID, "cot qkv"));
+  SAMPT_TRY(ws_get(c, &b.att, (size_t)M * CT_HID, "cot att"));
+  SAMPT_TRY(ws_get(c, &b.mlp, (size_t)M * 4 * CT_HID, "cot mlp"));
+  b.h16 = b.att16 = b.mlp16 = nullptr;
+  if (tc) {
+    SAMPT_TRY(ws_get(c, &b.h16, (size_t)M * 2 * CT_HID, "cot h16"));
+    SAMPT_TRY(ws_get(c, &b.att16, (size_t)M * 2 * CT_HID, "cot att16"));
+    SAMPT_TRY(ws_get(c, &b.mlp16, (size_t)M * 8 * CT_HID, "cot mlp16"));
+  }
+  if (kind == 0) return attn_block(c, st, w, b, tc != 0, M, N, S, S, 1);
+  return attn_block(c, st, w, b, tc != 0, M, S, N, 1, S);
+}
+
+extern "C" int sampt_test_cotracker_update(sampt_ctx* ctx, const float* delta, float* coords, float* ffeats, int N, float* vis_out,
+                                           void* stream) {
+  Ctx* c = reinterpret_cast<Ctx*>(ctx);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SAMPT_CHECK(N >= 1, "sampt_test_cotracker_update: no points");
+  CotHeadW hw;
+  SAMPT_TRY(load_head(c, &hw));
+  const PipsWin w = cot_win(nullptr, nullptr, nullptr, nullptr, 0, 0, nullptr, coords, ffeats, N);
+  SAMPT_TRY(cot_update(c, st, w, delta, hw));
+  return cot_vis(c, st, w, hw, vis_out);
 }
