@@ -1,17 +1,21 @@
 // Tensor-core GEMM for the SAM ViT encoder:  C[M,N] = epilogue( A[M,K] . B[N,K]^T ),  fp16/bf16 operands, fp32 accumulate.
 //
-// sm_90a design (one CTA per 128x128 output tile, 288 threads):
-//   warp 8          TMA producer : cp.async.bulk.tensor 2-D boxes (64 halves x rows, 128B swizzle) into a 5-stage smem ring,
+// sm_90a design (one CTA per 128x128 output tile, 288 threads, TWO CTAs per SM):
+//   warp 8          TMA producer : cp.async.bulk.tensor 2-D boxes (64 halves x rows, 128B swizzle) into a 3-stage smem ring,
 //                                  completion on per-stage mbarriers
 //   warpgroups 0,1  consumers    : wgmma.mma_async m64n128 (k16 fp16/bf16, k32 e4m3) on 64 rows each, fp32 accumulators in
 //                                  registers, one k-block in flight; then bias / GELU / residual / fp16|fp32|split store
+// Two resident CTAs (97 KB of shared memory and <= 112 registers per thread each) let one CTA's epilogue -- for the ViT's lin1
+// the GELU and the fp16 + two e4m3 stores take as long as its MMAs -- run while the other CTA keeps the tensor pipe busy.
 //
 // "Split" precision (accuracy dial, DESIGN.md §precision): an operand x is carried as fp16 hi + fp16 lo
 // (lo = fp16(x - hi)); the K loop then runs over up to three segments  A_hi.B_hi + A_lo.B_hi + A_hi.B_lo  accumulating
 // into the same registers.  Segments are described by column offsets into the A / B matrices, so the kernel is the same.
-// e4m3 segments (precision 6, tc_api.cuh) accumulate into a SEPARATE register tile that is added in the epilogue: wgmma's
-// fp8 accumulation does not keep full fp32 precision, which is harmless for the 2^-12-sized correction terms alone but would
-// round away the low bits of the fp16 main product if they shared one accumulator.
+// e4m3 segments (precision 6, tc_api.cuh) run FIRST, into the zeroed accumulator, and the fp16 segments after them: wgmma's
+// fp8 accumulation does not keep full fp32 precision, which is harmless while the accumulator holds only the 2^-12-sized
+// correction terms but would round away the low bits of the fp16 main product if that were already in it.  The fp16 wgmmas
+// then add at fp32 on top.  gemm_tc() reorders the caller's segments so (the sum does not depend on the order); one register
+// tile instead of two is what fits two CTAs on an SM.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "kernels.cuh"
@@ -22,15 +26,14 @@ namespace sampt {
 
 using namespace tc;
 
-constexpr int G_BM = 128, G_BN = 128, G_BK = 64, G_STAGES = 5;
+constexpr int G_BM = 128, G_BN = 128, G_BK = 64, G_STAGES = 3;
 constexpr int G_A_BYTES = G_BM * G_BK * 2;  // 16 KB
 constexpr int G_B_BYTES = G_BN * G_BK * 2;  // 16 KB
 constexpr int G_STAGE_BYTES = G_A_BYTES + G_B_BYTES;
 constexpr int G_SMEM_BYTES = G_STAGES * G_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 constexpr int G_THREADS = 288;
 
-template <bool F8>
-__global__ void __launch_bounds__(G_THREADS, 1)
+__global__ void __launch_bounds__(G_THREADS, 2)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
                GemmSeg seg, GemmEpi ep) {
   if (ep.skip != nullptr && *ep.skip != 0) return;   // uniform over the grid
@@ -78,13 +81,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // -------------------------------------------------------------- consumers: warpgroup g owns rows [64 g, 64 g + 64)
   const int g = warp >> 2, w = warp & 3;
   float acc[64];
-  float acc8[64];   // e4m3 segments (dead when !F8)
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = acc8[i] = 0.f;
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
   uint32_t it = 0;
   int prev_s = -1;
   for (int sg = 0; sg < seg.nseg; ++sg) {
-    const bool f8 = F8 && seg.f8[sg] != 0;
+    const bool f8 = seg.f8[sg] != 0;
     for (int kb = 0; kb < seg_kb[sg]; ++kb, ++it) {
       const int s = it % G_STAGES;
       mbar_wait(&full_bar[s], (it / G_STAGES) & 1);
@@ -94,7 +96,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_fence();
       if (f8) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_m64n128k32_e4m3(acc8, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
+        for (int k = 0; k < 4; ++k) wgmma_m64n128k32_e4m3(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
       } else if (ep.is_bf16) {
 #pragma unroll
         for (int k = 0; k < 4; ++k) wgmma_m64n128k16_bf16(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
@@ -110,7 +112,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   wgmma_wait<0>();
   wgmma_fence_regs(acc);
-  if (F8) wgmma_fence_regs(acc8);
 
   // -------------------------------------------------------------- epilogue straight from the accumulator registers
   const float acc_scale = ep.acc_scale ? __ldg(ep.acc_scale) : 1.0f;
@@ -127,7 +128,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int n = n_blk * G_BN + 8 * i + c2;
       if (n >= N) continue;   // N % 8 == 0: the pair is in or out together
       float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
-      if (F8) { v0 += acc8[4 * i + 2 * h]; v1 += acc8[4 * i + 2 * h + 1]; }
       v0 *= acc_scale; v1 *= acc_scale;
       if (ep.bias) { v0 += __ldg(ep.bias + n); v1 += __ldg(ep.bias + n + 1); }
       if (ep.act == 1) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
@@ -184,13 +184,15 @@ int gemm_tc(Ctx* c, cudaStream_t st, const void* A, int lda, const void* B, int 
   SAMPT_TRY(make_tmap_2d_f16(&tmB, B, (uint64_t)ldb, (uint64_t)N, (uint64_t)ldb * 2, G_BK, G_BN));
   const int m_tiles = (M + G_BM - 1) / G_BM, n_tiles = (N + G_BN - 1) / G_BN;
   const int grid = m_tiles * n_tiles;
-  if (f8) {
-    SAMPT_TRY(ensure_func_smem(c, "gemm_tc_kernel<f8>", gemm_tc_kernel<true>, G_SMEM_BYTES));
-    gemm_tc_kernel<true><<<grid, G_THREADS, G_SMEM_BYTES, st>>>(tmA, tmB, M, N, K, seg, ep);
-  } else {
-    SAMPT_TRY(ensure_func_smem(c, "gemm_tc_kernel", gemm_tc_kernel<false>, G_SMEM_BYTES));
-    gemm_tc_kernel<false><<<grid, G_THREADS, G_SMEM_BYTES, st>>>(tmA, tmB, M, N, K, seg, ep);
-  }
+  // e4m3 segments first (see the header), each group in the caller's order
+  GemmSeg ord{};
+  ord.nseg = seg.nseg;
+  int j = 0;
+  for (int pass = 1; pass >= 0; --pass)
+    for (int i = 0; i < seg.nseg; ++i)
+      if ((seg.f8[i] != 0) == (pass == 1)) { ord.a_off[j] = seg.a_off[i]; ord.b_off[j] = seg.b_off[i]; ord.f8[j] = seg.f8[i]; ++j; }
+  SAMPT_TRY(ensure_func_smem(c, "gemm_tc_kernel", gemm_tc_kernel, G_SMEM_BYTES));
+  gemm_tc_kernel<<<grid, G_THREADS, G_SMEM_BYTES, st>>>(tmA, tmB, M, N, K, ord, ep);
   c->launches++;
   SAMPT_LAUNCH_CHECK();
   return 0;

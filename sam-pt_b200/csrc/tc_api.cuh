@@ -24,7 +24,8 @@ struct GemmEpi {
 
 // K-loop segments for split precision: segment i multiplies A[:, a_off[i] : a_off[i]+K] with B[:, b_off[i] : b_off[i]+K]
 // (offsets in fp16 units).  f8[i] != 0: the segment's operands are e4m3 BYTES (K of them = K/2 fp16 units starting at the
-// offset), multiplied with wgmma e4m3 at twice the fp16 rate into a second fp32 accumulator that the epilogue adds.
+// offset), multiplied with wgmma e4m3 at twice the fp16 rate.  gemm_tc issues every e4m3 segment before the fp16 ones into the
+// one fp32 accumulator (gemm_tc.cu), whatever order the caller lists them in.
 struct GemmSeg { int nseg; int a_off[3]; int b_off[3]; int f8[3]; };
 
 // fp8-corrected split GEMM ("precision 6"), operand rows of 2K fp16 units:
