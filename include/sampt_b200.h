@@ -118,9 +118,10 @@ int sampt_attention_f16(sampt_ctx* ctx, const void* Qx, const void* Kx, const vo
                         int HD, int NT, int nheads, void* out, int ld_out, int split_off, void* stream);
 
 /* ---- unit-test entries, not used by the Python package -------------------------------------------------------------- */
-/* Twenty-six entries in all.  Here: the ViT's tensor-core GEMM and attention block, four stages of the SAM prompt encoder / mask
- * decoder (attention cores, prompt encoder, upscaling tail, postprocess + refinement control), five of the PIPS tracker and five
- * of the CoTracker window.  The five TinyViT and five PIPS++ entries are declared in their own sections. */
+/* Thirty entries in all.  Here: the ViT's tensor-core GEMM and attention block, four stages of the SAM ViT encoder (patch
+ * embedding, LayerNorm rows, one block, neck), four stages of the SAM prompt encoder / mask decoder (attention cores, prompt
+ * encoder, upscaling tail, postprocess + refinement control), five of the PIPS tracker and five of the CoTracker window.  The
+ * five TinyViT and five PIPS++ entries are declared in their own sections. */
 /* The ViT's tensor-core GEMM (csrc/gemm_tc.cu, csrc/tc_api.cuh) with every option the pipelines use:
  * C = epilogue(sum over segments i < nseg of A[:, a_off[i] : +K] . B[:, b_off[i] : +K]^T)   (offsets in fp16 units; f8[i] != 0:
  * the segment holds K e4m3 bytes).  a_off_host / b_off_host / f8_host are HOST int[nseg].  Epilogue, in this order: times
@@ -140,6 +141,30 @@ int sampt_test_gemm_tc(sampt_ctx* ctx, const void* A, int lda, const void* B, in
 int sampt_test_vit_attention(sampt_ctx* ctx, const void* qkv, const float* rel_pos_h, const float* rel_pos_w, int nwb, int nheads,
                              int S, int D, int DK, int Lkp, void* Qx, void* Kx, void* Vt, void* out, int ld_out, int split_off,
                              int out_f8, void* stream);
+/* Four stages of the SAM ViT encoder (csrc/vit_pipeline.cu) through the launchers of sampt_vit_encode, with the registered
+ * "sam.image_encoder.*" weights; precision 1..6 as in sampt_vit_encode.  Work buffers come from the ViT slab
+ * (sampt_ctx_set_vit_workspace).  Token rows are b*G*G + y*G + x, G = img_size / patch_size.
+ * embed: the patch embedding + pos_embed.  image = resized uint8 frames (B,3,Hr,Wr) (is_f32 = 0: normalised with the HOST mean3 /
+ *   std3, zero-padded to img_size^2) or the preprocessed float image (B,3,img_size,img_size) (is_f32 = 1; Hr, Wr, mean3, std3
+ *   unused) -> x_out [B*G*G, embed_dim] fp32; a_out (or NULL) [B*G*G, 3 P^2 * asp] fp16 receives the im2col operand, column
+ *   c*P*P + iy*P + ix, hi | lo (lo at column 3 P^2) at precisions 3..6 (asp = 2), hi alone at 1 and 2.
+ * ln: ln_rows on x [*, ldx] fp32: out row r from x row src[r] (device int[M] or NULL = r; src[r] < 0: a zero row); normalize 1 =
+ *   LayerNorm(gamma, beta, the blocks' eps 1e-6), 0 = cast only.  layout 0: out [M, D] fp16; 1: [M, 2D] fp16 hi | lo; 2: [M, 2D] fp16 units
+ *   = fp16 hi, then D e4m3 bytes of (v - hi) 2^12, then D e4m3 bytes of v 2^-3.
+ * block: sam.image_encoder.blocks.<blk> (global attention over the G x G grid when is_global, else window_size windows) on x
+ *   [B*G*G, embed_dim] in place; x_mid (or NULL) receives x after the attention half.  live_only != 0 (windowed only): the
+ *   padding-window skip's compacted form for resized Hr x Wr frames -- only the windows / tokens that reach the image are
+ *   computed, every other row of x is left as it was.
+ * neck: x [B*G*G, embed_dim] -> features (B, out_chans, G, G) fp32. */
+int sampt_test_vit_embed(sampt_ctx* ctx, const void* image, int is_f32, int B, int Hr, int Wr, int embed_dim, int img_size,
+                         int patch_size, int precision, const float* mean3, const float* std3, void* a_out, float* x_out,
+                         void* stream);
+int sampt_test_vit_ln(sampt_ctx* ctx, const float* x, int ldx, const int* src, int M, int D, int normalize, const float* gamma,
+                      const float* beta, int layout, void* out, void* stream);
+int sampt_test_vit_block(sampt_ctx* ctx, int blk, int is_global, float* x, float* x_mid, int B, int Hr, int Wr, int live_only,
+                         int embed_dim, int num_heads, int window_size, int img_size, int patch_size, int precision, void* stream);
+int sampt_test_vit_neck(sampt_ctx* ctx, const float* x, int B, int embed_dim, int img_size, int patch_size, int out_chans,
+                        int precision, float* features, void* stream);
 /* One SAM decoder attention core (csrc/decoder.cu), 8 heads, on caller-owned fp32 buffers, scale 1/sqrt(head dim):
  *   kind 0: token self-attention, block per (token, head) (the decode chain's kernel for T <= 16), head dim 32: q, k, v,
  *           out [T, 256], Nk == T;
@@ -231,7 +256,8 @@ int sampt_pil_resize_u8(sampt_ctx* ctx, const uint8_t* in, int B, int H, int W, 
  * HOST arrays.  precision: 1/2 as in sampt_gemm_f16 for every GEMM; 3 = 3 split passes for the MLP / patch-embed / neck GEMMs
  * and 2 (weights split) for qkv / proj, whose activations are fp16-limited by the attention path; 4 = 3 passes everywhere;
  * 5 = 3 passes except qkv (2); 6 = like 4 with the correction passes of qkv / lin1 / lin2 in e4m3 (sampt_gemm_f8c; needs the
- * "<layer>.w8" / ".w8s" tensors registered).  Replaces SamPredictor.set_image's encoder call (sam_pt.py:849). */
+ * "<layer>.w8" / ".w8s" tensors registered).  Every other GEMM reads "<layer>.w16", the fp16 hi (| lo) of w 2^s, and multiplies
+ * its accumulator by "<layer>.w16s" = 2^-s.  Replaces SamPredictor.set_image's encoder call (sam_pt.py:849). */
 int sampt_vit_encode(sampt_ctx* ctx, const uint8_t* resized_u8, int B, int Hr, int Wr, int depth, int embed_dim, int num_heads,
                      int window_size, const int* global_idx_host, int n_global, int img_size, int patch_size, int out_chans,
                      int precision, const float* pixel_mean_host, const float* pixel_std_host, float* features, float* interm,
@@ -263,8 +289,8 @@ int sampt_sam_predict_refine(sampt_ctx* ctx, const float* feat_tok, int G, const
 int sampt_vit_encode_f32(sampt_ctx* ctx, const float* x, int B, int depth, int embed_dim, int num_heads, int window_size,
                          const int* global_idx_host, int n_global, int img_size, int patch_size, int out_chans, int precision,
                          float* features, float* interm, void* stream);
-/* Forget the image-independent ViT rows saved by the experimental SAMPT_VIT_SKIP_PAD=1 path (csrc/vit_pipeline.cu); to be
- * called whenever the image-encoder weights are re-registered.  A no-op when that path is off. */
+/* Forget the image-independent ViT rows saved by the padding-window skip of sampt_vit_encode (csrc/vit_pipeline.cu; on unless
+ * SAMPT_VIT_SKIP_PAD=0); to be called whenever the image-encoder weights are re-registered.  A no-op when nothing is saved. */
 int sampt_vit_cache_clear(sampt_ctx* ctx);
 
 /* ---- TinyViT image encoder of MobileSAM / Light HQ-SAM (csrc/tinyvit.cu) ------------------------------------------------

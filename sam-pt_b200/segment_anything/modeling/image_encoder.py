@@ -64,13 +64,20 @@ class ImageEncoderViT(nn.Module):
 
     # ------------------------------------------------------------------ weights -> kernel-native layouts
     @staticmethod
-    def _w16(w: torch.Tensor, split: bool) -> torch.Tensor:
+    def _w16(w: torch.Tensor, split: bool):
+        """fp16 operand of w 2^s (hi, or hi | lo with lo = fp16(w 2^s - hi)) and the accumulator scale 2^-s, where s puts
+        max|w| 2^s in [2^14, 2^15), so that (hi + lo) 2^-s restores w to 2^-22 |w|.  Unscaled, weights of size ~1/sqrt(K) leave
+        every lo an fp16 subnormal, which restores w only to 2^-25 absolute."""
         w = w.detach().float()
-        hi = w.half()
+        amax = float(w.abs().max())
+        s = 15 - (math.frexp(amax)[1] if amax > 0 else 0)
+        ws = w * (2.0 ** s)
+        hi = ws.half()
+        scale = torch.tensor([2.0 ** (-s)], dtype=torch.float32, device=w.device)
         if not split:
-            return hi.contiguous()
-        lo = (w - hi.float()).half()
-        return torch.cat([hi, lo], dim=1).contiguous()
+            return hi.contiguous(), scale
+        lo = (ws - hi.float()).half()
+        return torch.cat([hi, lo], dim=1).contiguous(), scale
 
     @staticmethod
     def _w8(w: torch.Tensor):
@@ -91,6 +98,36 @@ class ImageEncoderViT(nn.Module):
         packed = torch.cat([hi.view(torch.uint8), hi8, lo8], dim=1).contiguous()      # (N, 2K + K + K) bytes
         return packed.view(torch.float16), torch.tensor([2.0 ** (-s)], dtype=torch.float32, device=w.device)
 
+    def native_weights(self) -> Dict[str, torch.Tensor]:
+        """{name under "sam.image_encoder.": tensor} in the layouts csrc/vit_pipeline.cu reads at self.precision: every GEMM
+        weight as "<layer>.w16" (fp16 w 2^s, hi | lo from precision 2 on) with its scale 2^-s as "<layer>.w16s", at precision
+        6 also the fp8-corrected "<layer>.w8" / ".w8s" of the block linears."""
+        split_b = self.precision >= 2   # (3, 4, 5: activations split as well, decided inside sampt_vit_encode)
+        sd = self.state_dict()
+        D, C = self.embed_dim, self.out_chans
+        out: Dict[str, torch.Tensor] = {}
+
+        def w16(name, w):
+            out[name + ".w16"], out[name + ".w16s"] = self._w16(w, split_b)
+
+        w16("patch_embed", sd["patch_embed.proj.weight"].reshape(D, -1))
+        out["patch_embed.proj.bias"] = sd["patch_embed.proj.bias"].float()
+        out["pos_embed"] = sd["pos_embed"].float().reshape(-1, D)
+        for i in range(self.depth):
+            b = f"blocks.{i}."
+            for n in ("norm1.weight", "norm1.bias", "norm2.weight", "norm2.bias", "attn.qkv.bias", "attn.proj.bias",
+                      "attn.rel_pos_h", "attn.rel_pos_w", "mlp.lin1.bias", "mlp.lin2.bias"):
+                out[b + n] = sd[b + n].float()
+            for n in ("attn.qkv", "attn.proj", "mlp.lin1", "mlp.lin2"):
+                w16(b + n, sd[b + n + ".weight"])
+                if self.precision == 6:
+                    out[b + n + ".w8"], out[b + n + ".w8s"] = self._w8(sd[b + n + ".weight"])
+        w16("neck.0", sd["neck.0.weight"].reshape(C, D))
+        w16("neck.2", sd["neck.2.weight"].permute(0, 2, 3, 1).reshape(C, 9 * C))
+        for n in ("neck.1.weight", "neck.1.bias", "neck.3.weight", "neck.3.bias"):
+            out[n] = sd[n].float()
+        return out
+
     def native_context(self, prefix: str = "sam.image_encoder.") -> native.Context:
         dev = self.pos_embed.device
         ctx = native.get_context(dev)
@@ -98,29 +135,8 @@ class ImageEncoderViT(nn.Module):
         if self._registered != key or not ctx.owns("sam.image_encoder", self):
             torch.cuda.synchronize(dev)  # nothing may still be reading the tensors this replaces
             native.check(native.lib().sampt_vit_cache_clear(ctx.handle), "vit_cache_clear")  # rows saved for the old weights
-            split_b = self.precision >= 2   # (3, 4, 5: activations split as well, decided inside sampt_vit_encode)
-            sd = self.state_dict()
-            D = self.embed_dim
-            ctx.set_tensor(prefix + "patch_embed.w16", self._w16(sd["patch_embed.proj.weight"].reshape(D, -1), split_b))
-            ctx.set_tensor(prefix + "patch_embed.proj.bias", sd["patch_embed.proj.bias"].float())
-            ctx.set_tensor(prefix + "pos_embed", sd["pos_embed"].float().reshape(-1, D))
-            for i in range(self.depth):
-                b = f"blocks.{i}."
-                for n in ("norm1.weight", "norm1.bias", "norm2.weight", "norm2.bias", "attn.qkv.bias", "attn.proj.bias",
-                          "attn.rel_pos_h", "attn.rel_pos_w", "mlp.lin1.bias", "mlp.lin2.bias"):
-                    ctx.set_tensor(prefix + b + n, sd[b + n].float())
-                for n in ("attn.qkv", "attn.proj", "mlp.lin1", "mlp.lin2"):
-                    ctx.set_tensor(prefix + b + n + ".w16", self._w16(sd[b + n + ".weight"], split_b))
-                if self.precision == 6:
-                    for n in ("attn.qkv", "attn.proj", "mlp.lin1", "mlp.lin2"):
-                        w8, w8s = self._w8(sd[b + n + ".weight"])
-                        ctx.set_tensor(prefix + b + n + ".w8", w8)
-                        ctx.set_tensor(prefix + b + n + ".w8s", w8s)
-            C = self.out_chans
-            ctx.set_tensor(prefix + "neck.0.w16", self._w16(sd["neck.0.weight"].reshape(C, D), split_b))
-            ctx.set_tensor(prefix + "neck.2.w16", self._w16(sd["neck.2.weight"].permute(0, 2, 3, 1).reshape(C, 9 * C), split_b))
-            for n in ("neck.1.weight", "neck.1.bias", "neck.3.weight", "neck.3.bias"):
-                ctx.set_tensor(prefix + n, sd[n].float())
+            for name, t in self.native_weights().items():
+                ctx.set_tensor(prefix + name, t)
             self._registered = key
             ctx.claim("sam.image_encoder", self)
         return ctx

@@ -385,13 +385,17 @@ def _random_segments(M, N, K, f8s, seed):
     return A, B, [(a_off[i], b_off[i], f8s[i]) for i in range(len(f8s))]
 
 
-# k-blocks per segment: K / 64 for fp16, K / 128 for e4m3; the producer / consumer ring has 5 stages
+# k-blocks per segment: K / 64 for fp16, K / 128 for e4m3; the producer / consumer ring has 3 stages.  gemm_tc issues the e4m3
+# segments first, whatever order the caller lists them in.
 @pytest.mark.parametrize("f8s,K", [
     ((0,), 64),            # 1 k-block
     ((1,), 128),           # 1
-    ((0, 1, 1), 128),      # 2 + 1 + 1 = 4 (below the ring depth)
-    ((0, 0, 1), 128),      # 2 + 2 + 1 = 5 (equal)
-    ((0,), 320),           # 5
+    ((0,), 128),           # 2 (below the ring depth)
+    ((0,), 192),           # 3 (equal)
+    ((0,), 256),           # 4 (one above)
+    ((1, 1), 128),         # 1 + 1 = 2
+    ((0, 1), 128),         # 2 + 1 = 3, e4m3 listed last
+    ((0, 0, 1), 128),      # 2 + 2 + 1 = 5, e4m3 listed last
     ((1, 0, 1), 256),      # 2 + 4 + 2 = 8
     ((1, 1, 0), 640),      # 5 + 5 + 10 = 20
     ((0, 0, 0), 320),      # 15

@@ -1,4 +1,4 @@
-"""CPU check of the index arithmetic behind the experimental SAMPT_VIT_SKIP_PAD path (csrc/vit_pipeline.cu): the three device
+"""CPU check of the index arithmetic behind the padding-window skip (csrc/vit_pipeline.cu): the three device
 map kernels are mirrored here formula by formula and checked for the properties the pipeline relies on (partition of the token
 grid, windows closed under the live set, constant tokens = tokens whose whole window is zero padding)."""
 import math
