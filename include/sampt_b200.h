@@ -425,6 +425,24 @@ int sampt_vos_index_masks(sampt_ctx* ctx, const float* logits, int M, int T, int
 int sampt_patch_filter(sampt_ctx* ctx, const uint8_t* frames, int T, int H, int W, const float* query, const float* traj,
                        int N, int patch_size, float threshold, float* vis, float* sim, void* stream);
 
+/* ---- interactive point correction (sam_pt/modeling/sam_pt_interactive.py) ------------------------------------------------- */
+/* DAVIS J&F (davis2017-evaluation db_eval_iou / db_eval_boundary) as exact counts for T frames in one call: logits [T,H,W]
+ * float32 (prediction P = logit > 0), gt [T,H,W] uint8 (G = gt != 0), radius = ceil(0.008 * |(H,W)|) (the caller computes it
+ * in float64 as numpy does), scratch >= 3*T*H*W + 2 bytes -> counts [T,8] int64 = |P&G|, |P|G|, |P|, |G|, |dP|, |dG|,
+ * |dP & dil(dG)|, |dG & dil(dP)| with d = _seg2bmap and dil = cv2.dilate with skimage.morphology.disk(radius). W <= 16384. */
+int sampt_jf_counts(sampt_ctx* ctx, const float* logits, const uint8_t* gt, int T, int H, int W, int radius, uint8_t* scratch,
+                    long long* counts, void* stream);
+/* Point categories of sam_pt_interactive.py:341-356: logits [H,W], gt [H,W] u8, xy [n,2] float32 (x,y), labels [n] int32 ->
+ * out [n] int32 = tp | tn<<1 | fp<<2 | fn<<3 | correct<<4 sampled at (rint(y), rint(x)); a negative index wraps as in Python,
+ * an index still outside the image gives -1 (the caller raises IndexError before the call, as the reference does). */
+int sampt_point_categories(sampt_ctx* ctx, const float* logits, const uint8_t* gt, int H, int W, const float* xy, const int* labels,
+                           int n, int* out, void* stream);
+/* sklearn.cluster.DBSCAN(eps, min_samples).fit(pts).labels_ (sam_pt_interactive.py:706-707): pts [n,2] float32 holding integer
+ * pixel coordinates, scratch [3n] int32 -> labels [n] int32 (-1 = noise).  Neighbourhoods: squared distance <= eps*eps in
+ * float64, the point itself included; clusters numbered by their smallest core index; a border point takes the smallest label
+ * among its core neighbours. */
+int sampt_dbscan(sampt_ctx* ctx, const float* pts, int n, double eps, int min_samples, int* labels, int* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
