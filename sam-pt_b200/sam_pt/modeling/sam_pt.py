@@ -475,19 +475,62 @@ class SamPt(nn.Module):
           D. NCCL  : all-gather of the (T,N,3) trajectories/visibilities (a few KB)
           E. local : prompt + mask decode on the owned frames
         Returns, per clip, {"trajectories","visibilities","logits" (M, n_owned, H, W), "frame_ids", "scores_per_frame"}
-        (logits stay sharded unless gather_logits)."""
+        (logits stay sharded unless gather_logits).  Every tensor stays on the device (`outputs_on_cpu` is `forward`'s).
+        The masks of a clip are tracked `point_tracker_mask_batch_size` at a time, as `_track_points` does, so the results are
+        those of `forward` also for trackers whose points interact (CoTracker).  Outside the path and raising before any
+        launch: point re-initialisation, patch-matching filtering, queries given as masks, `target_hw` different from the
+        frame size, clips of different frame sizes, a tracker without `shard_features` / `track_on_features`.
+        The three local stages take (rank, world) explicitly, so that one process can run them for every rank in turn."""
         import torch.distributed as dist
         from sampt_b200 import sharding
         world, rank = dist.get_world_size(), dist.get_rank()
-        dev = self.device
-        trk = self.point_tracker.to(dev)
+        state = self._sharded_encode(videos, rank, world)                                           # A
+        fulls = sharding.allgather_clips(state["locs"], state["Ts"])                                # B (one collective for all clips)
+        slab = self._sharded_track(state, fulls, rank, world)                                       # C
+        del fulls
+        gathered = torch.empty((world,) + tuple(slab.shape), device=slab.device)                    # D (tiny)
+        dist.all_gather_into_tensor(gathered.view((world * slab.shape[0],) + tuple(slab.shape[1:])), slab)
+        results = self._sharded_decode(state, gathered, rank, world)                                # E
+        if gather_logits:
+            for c, T in enumerate(state["Ts"]):   # (clips may carry different numbers of masks: one collective per clip)
+                full = sharding.allgather_frames(results[c]["logits"].transpose(0, 1).contiguous(), T, clip=c)
+                results[c]["logits"] = full.transpose(0, 1)
+                results[c]["frame_ids"] = list(range(T))
+        return results
+
+    def _check_sharded_inputs(self, videos):
+        """What `forward` does and the frame-sharded path does not is refused here, before anything is uploaded or launched."""
+        trk = self.point_tracker
         if not (hasattr(trk, "shard_features") and hasattr(trk, "track_on_features")):
             raise NotImplementedError(f"{type(trk).__name__} has no frame-sharded path (needs shard_features / track_on_features)")
+        if self.use_point_reinit:
+            raise NotImplementedError("use_point_reinit is not built on the frame-sharded path (it re-tracks from SAM's own masks)")
+        if self.use_patch_matching_filtering:
+            raise NotImplementedError("use_patch_matching_filtering is not built on the frame-sharded path")
+        hw = tuple(videos[0]["image"][0].shape[-2:])
+        for c, v in enumerate(videos):
+            if v.get("query_points") is None:
+                raise NotImplementedError(f"clip {c}: the frame-sharded path takes query_points; query_masks are not sampled here")
+            if any(tuple(f.shape[-2:]) != hw for f in v["image"]):
+                raise ValueError(f"clip {c}: the frame-sharded path batches the frames of all clips, which must share one frame size "
+                                 f"({hw} in clip 0)")
+            if v.get("target_hw") is not None and tuple(int(x) for x in v["target_hw"]) != hw:
+                raise ValueError(f"clip {c}: target_hw {tuple(v['target_hw'])} differs from the frame size {hw}; the frame-sharded "
+                                 f"path returns masks and trajectories at the frame size only")
+
+    @torch.no_grad()
+    def _sharded_encode(self, videos, rank, world):
+        """Stage A on `rank` of `world`: upload the owned frames of every clip as one batch, start the SAM encoder on them and
+        run the tracker's encoder.  `locs[c]` = features of the owned frames of clip c (the all-gather payload)."""
+        from sampt_b200 import sharding
+        self._check_sharded_inputs(videos)
+        dev = self.device
+        trk = self.point_tracker.to(dev)
         C = len(videos)
         Ts = [len(v["image"]) for v in videos]
         own = [sharding.owned_frames(Ts[c], rank, world, c) for c in range(C)]
         h, w = videos[0]["image"][0].shape[-2:]
-        # A. upload only the owned frames (async from pinned memory), one batch for every clip
+        # upload only the owned frames (async from pinned memory), one batch for every clip
         specs = [(c, f) for c in range(C) for f in own[c]]
         if len(specs) == 0:
             all_own = torch.empty((0, 3, h, w), dtype=torch.uint8, device=dev)
@@ -499,47 +542,47 @@ class SamPt(nn.Module):
         for c in range(C):
             locs.append(fm_all[off:off + len(own[c])])
             off += len(own[c])
-        # B. the exchange step (one collective for all clips)
-        fulls = sharding.allgather_clips(locs, Ts)
-        # C. chains: clip c on rank c % world
-        tv_local, shapes = [], []
-        for c, v in enumerate(videos):
-            q = v["query_points"]
-            M, P, _ = q.shape
-            shapes.append((M, P))
-            if c % world == rank:
-                traj, vis = trk.track_on_features(fulls[c], q.reshape(1, M * P, 3).to(dev), (h, w))
-                tv_local.append(torch.cat([traj[0], vis[0].float()[..., None]], dim=-1))  # (T, N, 3)
-        del fulls
-        # D. share the trajectories (tiny)
-        N_max = max(m * p for m, p in shapes)
-        T_max = max(Ts)
-        n_slots = (C + world - 1) // world
-        slab = torch.zeros((n_slots, T_max, N_max, 3), device=dev)
-        for i, t in enumerate(tv_local):
-            slab[i, : t.shape[0], : t.shape[1]] = t
-        gathered = torch.empty((world * n_slots, T_max, N_max, 3), device=dev)
-        dist.all_gather_into_tensor(gathered, slab)
-        # E. SAM on the owned frames
+        return {"Ts": Ts, "own": own, "hw": (h, w), "specs": specs, "all_own": all_own, "pre": pre, "locs": locs,
+                "queries": [v["query_points"] for v in videos]}
+
+    @torch.no_grad()
+    def _sharded_track(self, state, fulls, rank, world):
+        """Stage C: the tracker chain of clip c on rank c % world, on the gathered features `fulls[c]` (T_c, H4, W4, 128).
+        Returns the (n_slots, T_max, N_max, 3) slab of (x, y, visibility) this rank contributes to the second all-gather:
+        slot i holds clip rank + i * world."""
+        dev = self.device
+        trk = self.point_tracker
+        Ts, queries = state["Ts"], state["queries"]
+        bs = self.point_tracker_mask_batch_size
+        N_max = max(q.shape[0] * q.shape[1] for q in queries)
+        slab = torch.zeros(((len(Ts) + world - 1) // world, max(Ts), N_max, 3), device=dev)
+        for c in range(rank, len(Ts), world):
+            q = queries[c]
+            P = q.shape[1]
+            parts = []
+            for i in range(0, q.shape[0], bs):   # the mask batches of _track_points: a CoTracker call mixes the points it is given
+                qb = q[i:i + bs].to(dev)
+                traj, vis = trk.track_on_features(fulls[c], qb.reshape(1, qb.shape[0] * P, 3), state["hw"])
+                parts.append(torch.cat([traj[0], vis[0].float()[..., None]], dim=-1))  # (T, m * P, 3)
+            tv = torch.cat(parts, dim=1)
+            slab[c // world, : tv.shape[0], : tv.shape[1]] = tv
+        return slab
+
+    @torch.no_grad()
+    def _sharded_decode(self, state, gathered, rank, world):
+        """Stage E: gathered (world, n_slots, T_max, N_max, 3) = the slabs of `_sharded_track` of every rank, in rank order;
+        out-of-frame relabel as in `_track_points`, then prompt + mask decode on the owned frames."""
+        h, w = state["hw"]
+        Ts = state["Ts"]
         clips = []
-        for c in range(C):
-            M, P = shapes[c]
-            tv = gathered[(c % world) * n_slots + c // world, : Ts[c], : M * P]
+        for c, q in enumerate(state["queries"]):
+            M, P, _ = q.shape
+            tv = gathered[c % world, c // world, : Ts[c], : M * P]
             traj = tv[..., :2].reshape(Ts[c], M, P, 2)
             vis = tv[..., 2].reshape(Ts[c], M, P)
             out_code = float(PointVisibilityType.OUTSIDE_FRAME.value)
             oob = (traj[..., 0] / w < 0.01) | (traj[..., 1] / h < 0.01) | (traj[..., 0] / w > 0.99) | (traj[..., 1] / h > 0.99)
             clips.append((traj, torch.where(oob, torch.full_like(vis, out_code), vis)))
-        decoded = self._apply_sam_multi(all_own, specs, clips, pre=pre)
-        results = []
-        for c in range(C):
-            logits, spf, _ = decoded[c]
-            res = {"trajectories": clips[c][0], "visibilities": clips[c][1], "logits": logits, "frame_ids": own[c],
-                   "scores_per_frame": spf}
-            results.append(res)
-        if gather_logits:
-            for c in range(C):   # (clips may carry different numbers of masks: one collective per clip)
-                full = sharding.allgather_frames(results[c]["logits"].transpose(0, 1).contiguous(), Ts[c], clip=c)
-                results[c]["logits"] = full.transpose(0, 1)
-                results[c]["frame_ids"] = list(range(Ts[c]))
-        return results
+        decoded = self._apply_sam_multi(state["all_own"], state["specs"], clips, pre=state["pre"])
+        return [{"trajectories": clips[c][0], "visibilities": clips[c][1], "logits": decoded[c][0], "frame_ids": state["own"][c],
+                 "scores_per_frame": decoded[c][1]} for c in range(len(Ts))]

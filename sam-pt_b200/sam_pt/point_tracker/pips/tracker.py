@@ -41,7 +41,11 @@ class PipsPointTracker(PointTracker):
     # ---- frame-sharded multi-GPU path (SamPt.forward_clips_sharded): encoder on the owned frames, chain on gathered features
     def shard_features(self, frames_u8):
         """(n,3,H,W) uint8 frames this rank owns -> (n,H/4,W/4,128) fp32 BasicEncoder features (the all-gather payload)."""
-        return self.model.fnet_frames(frames_u8.to(self.device))
+        frames_u8 = frames_u8.to(self.device)
+        if frames_u8.shape[0] == 0:   # a rank that owns no frame (more ranks than frames) contributes an empty payload
+            H, W = frames_u8.shape[-2:]
+            return torch.empty((0, H // 4, W // 4, 128), device=self.device, dtype=torch.float32)
+        return self.model.fnet_frames(frames_u8)
 
     def track_on_features(self, fmaps, query_points, frame_hw=None):
         """fmaps (T,H/4,W/4,128): every frame's features in frame order (after the all-gather); the pyramid is built locally."""

@@ -51,24 +51,39 @@ def allgather_clips(locals_: Sequence[torch.Tensor], Ts: Sequence[int], group=No
     """ONE collective for several clips: locals_[i] = (n_owned_i, ...) rows this rank owns of clip clips[i] (T_i frames).
     Returns, per clip, the (T_i, ...) tensor in frame order, on every rank."""
     world = dist.get_world_size(group)
-    rank = dist.get_rank(group)
+    slab = pack_clips(locals_, Ts, dist.get_rank(group), world, clips)
+    out = torch.empty((world,) + tuple(slab.shape), dtype=slab.dtype, device=slab.device)
+    dist.all_gather_into_tensor(out.view((world * slab.shape[0],) + tuple(slab.shape[1:])), slab, group=group)
+    return unpack_clips(out, Ts, world, clips)
+
+
+def pack_clips(locals_: Sequence[torch.Tensor], Ts: Sequence[int], rank: int, world: int,
+               clips: Sequence[int] | None = None) -> torch.Tensor:
+    """The slab `rank` contributes to the all-gather: per clip `padded_count` rows (its owned frames in increasing frame
+    order, then zeros), the clips one after the other -> (sum of the padded counts, ...).  No collective."""
     clips = list(range(len(locals_))) if clips is None else list(clips)
     ns = [padded_count(T, world) for T in Ts]
-    tail = tuple(locals_[0].shape[1:])
-    dev, dt = locals_[0].device, locals_[0].dtype
-    slab = torch.zeros((sum(ns),) + tail, dtype=dt, device=dev)
+    slab = torch.zeros((sum(ns),) + tuple(locals_[0].shape[1:]), dtype=locals_[0].dtype, device=locals_[0].device)
     off = 0
     for loc, T, c, n in zip(locals_, Ts, clips, ns):
         assert loc.shape[0] == len(owned_frames(T, rank, world, c)), (loc.shape, T, rank, world, c)
         slab[off:off + loc.shape[0]] = loc
         off += n
-    out = torch.empty((world, sum(ns)) + tail, dtype=dt, device=dev)
-    dist.all_gather_into_tensor(out.view((world * sum(ns),) + tail), slab, group=group)
+    return slab
+
+
+def unpack_clips(stacked: torch.Tensor, Ts: Sequence[int], world: int, clips: Sequence[int] | None = None) -> List[torch.Tensor]:
+    """stacked (world, sum of the padded counts, ...): the slabs of `pack_clips` of every rank, in rank order (what the
+    all-gather delivers) -> per clip the (T_i, ...) tensor in frame order.  No collective."""
+    clips = list(range(len(Ts))) if clips is None else list(clips)
+    assert stacked.shape[0] == world and stacked.shape[1] == sum(padded_count(T, world) for T in Ts), (stacked.shape, Ts, world)
+    tail = tuple(stacked.shape[2:])
     res = []
     off = 0
-    for T, c, n in zip(Ts, clips, ns):
-        block = out[:, off:off + n].reshape((world * n,) + tail)           # row r*n + i = i-th owned frame of rank r
-        idx = torch.tensor(_gather_index(T, world, c, n), device=dev)
+    for T, c in zip(Ts, clips):
+        n = padded_count(T, world)
+        block = stacked[:, off:off + n].reshape((world * n,) + tail)       # row r*n + i = i-th owned frame of rank r
+        idx = torch.tensor(_gather_index(T, world, c, n), device=stacked.device)
         res.append(block.index_select(0, idx))
         off += n
     return res

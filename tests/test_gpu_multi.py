@@ -43,14 +43,19 @@ def _worker(rank, world, port, tmp, ret, tracker="pips"):
                                  device=torch.device("cuda", rank), cotracker_state_dict=cot_sd, cotracker_interp_shape=(64, 96))
     # ragged: 9 and 11 frames over 2 ranks, 3 clips (more clips than ranks), ownership rotated per clip
     videos = [synth.make_video_dict(9 + 2 * (c % 2), 96, 128, 4, seed=80 + c) for c in range(world + 1)]
+    # 6 masks > point_tracker_mask_batch_size = 5, queried on different frames: the chain tracks 5 + 1 masks as forward does
+    clip = synth.make_clip(10, 96, 128, seed=89)
+    videos.append({"image": [f for f in clip["frames"]], "target_hw": (96, 128),
+                   "query_points": torch.cat([synth.make_query_points(clip, 4, 89 + m, t=t) for m, t in enumerate((0, 3, 9, 0, 5, 2))])})
     res = model.forward_clips_sharded(videos, gather_logits=True)
     ok = True
     for c, v in enumerate(videos):
+        # bitwise: the encoders are batch invariant and the chain runs the calls forward runs (test_gpu_sharded_one_gpu.py
+        # establishes both on one device); empty masks are -inf on both sides, which torch.equal compares equal
         single = model(v)
-        ok &= bool((res[c]["trajectories"].cpu() - single["trajectories"].cpu()).abs().max() < 1e-4)
+        ok &= bool(torch.equal(res[c]["trajectories"].cpu(), single["trajectories"].cpu()))
         ok &= bool(torch.equal(res[c]["visibilities"].cpu(), single["visibilities"].cpu()))
-        a, b = res[c]["logits"][0].cpu() > 0, single["logits"][0].cpu() > 0
-        ok &= bool(((a & b).sum().float() / (a | b).sum().clamp(min=1).float()) >= 0.999)
+        ok &= bool(torch.equal(res[c]["logits"].cpu(), torch.stack(single["logits"]).cpu()))
     t = torch.tensor([1.0 if ok else 0.0], device="cuda")
     dist.all_reduce(t, op=dist.ReduceOp.MIN)
     if rank == 0:

@@ -33,6 +33,14 @@ def _worker(rank, world, port, T, ret):
     locs = [fulls[c][sharding.owned_frames(t, rank, world, c)] for c, t in enumerate(Ts)]
     gots = sharding.allgather_clips(locs, Ts)
     ok = ok and all(torch.equal(g, f) for g, f in zip(gots, fulls))
+    # the collective delivers exactly the stack of every rank's pack_clips slab: unpack_clips of that stack, with no
+    # collective, is what allgather_clips returned (the one-GPU virtual-rank test of the sharded path rests on this)
+    stacked = torch.stack([sharding.pack_clips([fulls[c][sharding.owned_frames(t, r, world, c)] for c, t in enumerate(Ts)], Ts, r, world)
+                           for r in range(world)])
+    ok = ok and all(torch.equal(g, u) for g, u in zip(gots, sharding.unpack_clips(stacked, Ts, world)))
+    # the same with an explicit clip rotation (allgather_frames(..., clip=c) of gather_logits)
+    rot = sharding.allgather_clips([fulls[0][sharding.owned_frames(Ts[0], rank, world, 3)]], Ts[:1], clips=[3])
+    ok = ok and torch.equal(rot[0], fulls[0])
     t = torch.tensor([1.0 if ok else 0.0])
     dist.all_reduce(t, op=dist.ReduceOp.MIN)
     # max-over-ranks timing reduction used by bench.py
@@ -72,6 +80,31 @@ def test_allgather_frames_world4_ragged():
         assert p.exitcode == 0
     ok, ms = ret.get(timeout=10)
     assert ok == 1.0 and ms == 10.0 + world - 1
+
+
+def test_pack_unpack_clips_reproduce_the_frames():
+    """pack_clips / unpack_clips are the two halves of allgather_clips around its collective: stacking every rank's slab and
+    unpacking gives back every clip in frame order, for world 1...9 and T 1...20 (T < world: ranks that own nothing), with the
+    default clip numbering and with an explicit rotation; the padding rows are zero."""
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    sys.path.insert(0, os.path.join(root, "sam-pt_b200"))
+    from sampt_b200 import sharding
+    for world in range(1, 10):
+        for T in range(1, 21):
+            Ts = [T, 21 - T, 7]
+            fulls = [torch.arange(t * 6, dtype=torch.float32).reshape(t, 2, 3) + 1000 * (i + 1) for i, t in enumerate(Ts)]
+            for clips in (None, [5, 0, 2 * world + 1]):
+                ids = list(range(len(Ts))) if clips is None else clips
+                slabs = []
+                for r in range(world):
+                    own = [sharding.owned_frames(t, r, world, c) for t, c in zip(Ts, ids)]
+                    slab = sharding.pack_clips([f[o] for f, o in zip(fulls, own)], Ts, r, world, clips)
+                    assert slab.shape == (sum(sharding.padded_count(t, world) for t in Ts), 2, 3)
+                    assert int((slab != 0).any(dim=2).any(dim=1).sum()) == sum(len(o) for o in own)   # the rest is padding
+                    slabs.append(slab)
+                got = sharding.unpack_clips(torch.stack(slabs), Ts, world, clips)
+                assert all(torch.equal(g, f) for g, f in zip(got, fulls)), (world, T, clips)
 
 
 def test_owned_frames_partition_every_world_size():
